@@ -1,16 +1,18 @@
 #!/usr/bin/env python
-"""bench.py — frames/s of the full ThinkTwice forward (4 cams x 2 sweeps + LiDAR, K=5) on N B200.
+"""bench.py — frames/s of the full ThinkTwice forward (4 cams x 2 sweeps + LiDAR, K=5) on N H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference] [--dump-outputs DIR]
 
 One JSON line on rank 0 (contract in the task statement):
   value      : frames/s, whole job, inputs already resident in HBM (device-timed, max over ranks)
   e2e        : same metric through the public API with HOST (pinned) inputs, H2D + D2H inside the timed region
   roofline   : dominant kernel family (implicit-GEMM convolution), algorithmic FLOPs / CUDA-event time, vs the
-               measured dense tensor peak of MEASURED_PEAKS.json
+               measured dense tensor peak of MEASURED_PEAKS.json (else the H100 SXM data-sheet figure)
   cpu_baseline: the oracle (plain-PyTorch restatement of the reference forward, incl. its dead work) on the host cores
 `--impl reference` times that CPU restatement alone (the reference itself cannot be imported here: mmcv/mmdet3d/
 spconv are absent — DESIGN.md), rank 0 only.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step as DIR/<name>.npy (float32; arrays larger
+than 2^20 elements as a fixed seeded sample of their flattened elements), so that two builds can be compared output for output.
 """
 import argparse
 import json
@@ -24,7 +26,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 METRIC = json.load(open(os.path.join(ROOT, 'BASELINE.json')))['metric'] if os.path.exists(os.path.join(ROOT, 'BASELINE.json')) else \
-    'frames/sec full encoder+decoder fwd (4-cam+LiDAR, 200\u00d7200 BEV) at 1/2/4/8 B200'
+    'frames/sec full encoder+decoder fwd (4-cam+LiDAR, 200\u00d7200 BEV) at 1/2/4/8 H100'
 SHAPE = ('thinktwice.py config, 4 cams x 2 sweeps 448x896 + 40k-point LiDAR, K=5 decoder '
          '(the config file yields a 21x21 camera BEV / 84x84 LiDAR BEV, not 200x200: SURVEY.md fact 3)')
 
@@ -68,7 +70,7 @@ def load_peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return j['bf16_tflops_sustained'], j['hbm_gbs'], 'measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)'
-    return 1400.0, 6650.0, 'fallback (B200_PROFILING.md)'
+    return 989.0, 3350.0, 'H100 SXM data sheet (dense FP16 / BF16, HBM3), not a measurement'
 
 
 def cpu_oracle_worker(max_frames):
@@ -169,12 +171,40 @@ def cpu_oracle(max_frames, budget_s):
     return fps, len(frames), threads or 0, note
 
 
+DUMP_BUDGET = 64 << 20          # bytes of .npy payload --dump-outputs may write
+DUMP_SAMPLE = 1 << 20           # larger arrays are reduced to this many elements
+
+
+def dump_outputs(pred, gathered, out_dir):
+    """the arrays a caller of forward_inference received in the last timed step, as float32 .npy files (plus the gathered
+    waypoints of a multi-GPU run).  An array of more than DUMP_SAMPLE elements is written as the elements at a fixed set of
+    flattened positions (seeded, sorted) so that runs with the same arguments stay comparable element for element."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: pred[k] for k in pred.keys() if torch.is_tensor(pred[k])}
+    if gathered is not None:
+        arrays['gathered_pred_wp'] = gathered
+    total = 0
+    for name in sorted(arrays):
+        t = arrays[name].detach().float()
+        if t.numel() > DUMP_SAMPLE:
+            gen = torch.Generator(device='cpu').manual_seed(0)
+            idx = torch.randperm(t.numel(), generator=gen)[:DUMP_SAMPLE].sort().values
+            t, name = t.reshape(-1)[idx.to(t.device)], f'{name}.sample'
+        a = t.cpu().numpy().astype(np.float32)
+        total += a.nbytes
+        if total > DUMP_BUDGET:
+            raise RuntimeError(f'--dump-outputs: more than {DUMP_BUDGET >> 20} MB of outputs')
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
-    ap.add_argument('--batch', type=int, default=32, help='frames per GPU per step (32 = the throughput configs[2] / configs[3])')
+    ap.add_argument('--batch', type=int, default=16, help='frames per GPU per step (16 = the throughput configs[2] / configs[3]; 32 exceeds 80 GB)')
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference', 'reference-worker', 'make-weights'])
     ap.add_argument('--out', default=None, help='(make-weights) checkpoint file to write')
     ap.add_argument('--no-cpu-baseline', action='store_true')
@@ -182,9 +212,11 @@ def main():
     ap.add_argument('--no-graph', action='store_true', help='launch every kernel from the host instead of replaying a CUDA graph')
     ap.add_argument('--dump-convs', default=None, help='write per-conv-launch (name, flops, ms) of one step to this JSON file')
     ap.add_argument('--conv', default='f16s', choices=['simt', '3xtf32', 'tf32', 'f16s'],
-                    help='dense-conv engine: tcgen05 scaled-split fp16 (fp32-class, default), tcgen05 3xTF32, single-pass TF32, or SIMT fp32')
-    ap.add_argument('--dbg', type=int, default=0, help='experiment: tt_debug_set knob bits (see csrc/gemm_conv_tc.cu)')
-    ap.add_argument('--tc-reserve', type=int, default=0, help='experiment: SMs the persistent tcgen05 kernels leave free for the side branch')
+                    help='dense-conv engine: tensor-core scaled-split fp16 (fp32-class, default), tensor-core 3xTF32, single-pass TF32, or SIMT fp32')
+    ap.add_argument('--dbg', type=int, default=0, help='experiment: tt_debug_set knob bits, bit 7 and up shifted as documented in include/tt_b200.h (unknown bits fail)')
+    ap.add_argument('--tc-reserve', type=int, default=0, help='experiment: SMs the persistent tensor-core kernels leave free for the side branch')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32, at most 64 MB in all)')
     args = ap.parse_args()
     rank, world = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1))
     local_rank = int(os.environ.get('LOCAL_RANK', 0))
@@ -201,7 +233,7 @@ def main():
             'config': {'workload': workload(args.batch, args.gpus), 'frames_per_gpu_per_step': args.batch, 'global_batch': args.batch * args.gpus,
                        'refine_num': 5, 'conv_engine': args.conv, 'cuda_graph': not args.no_graph,
                        'parallelism': f'dp{args.gpus} (frames sharded, one NCCL all_gather of pred_wp)',
-                       'l2': 'per-step working set (0.5 GB weights + >1 GB activations per frame) exceeds the 126 MB L2; no explicit flush'}}
+                       'l2': 'per-step working set (0.5 GB weights + >1 GB activations per frame) exceeds the 50 MB L2; no explicit flush'}}
 
     if args.impl == 'reference':
         if rank != 0:
@@ -239,8 +271,11 @@ def main():
     from thinktwice_b200.parallel import gather_waypoints
     gathered = torch.empty(world * B, 6, 4, 2, device=dev) if world > 1 else None
 
+    last = {}
+
     def step(batch):
         pred = model.forward_inference(batch)
+        last['pred'] = pred
         wp = pred['pred_wp']
         if world > 1:                                            # the path's single collective: gather of the waypoints
             return gather_waypoints(wp, world, out=gathered)
@@ -265,7 +300,7 @@ def main():
         return float(ms.item())
 
     if args.tc_reserve or args.dbg:
-        lib.load().tt_debug_set((args.tc_reserve << 8) | (args.dbg & 0xFF) | ((args.dbg >> 8) << 16))
+        lib.check(lib.load().tt_debug_set((args.tc_reserve << 8) | (args.dbg & 0xFF) | ((args.dbg >> 8) << 16)), 'tt_debug_set')
     n_eager = lib.launch_count()
     step(resident)                                               # eager step: allocates every buffer, counts launches
     torch.cuda.synchronize()
@@ -279,6 +314,8 @@ def main():
     th = threading.Thread(target=clocks_sampler, args=(stop, samples, local_rank), daemon=True)
     th.start()
     ms = timed(resident, args.steps, read_back=False)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(last['pred'], gathered if world > 1 else None, args.dump_outputs)
     launches = launches_per_step * args.steps                    # graph replays execute the same kernel nodes every step
     for _ in range(max(args.warmup, 3)):                         # the host-input path has its own graphs / buffers: warm them outside the timed region
         step(host).cpu()
@@ -326,16 +363,6 @@ def main():
         json.dump([(n, f, a.elapsed_time(b)) for (n, f, a, b) in model.eng.prof], open(args.dump_convs, 'w'))
     model.eng.prof = None
     tensor_peak, hbm_peak, peak_src = load_peaks()
-    traffic, traffic_note = None, None
-    tpath = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'r2_kernels_b1.json')
-    if os.path.exists(tpath):                                    # DRAM bytes per launch from the committed ncu --set full capture
-        tj = json.load(open(tpath))
-        dom = [l for l in tj['launches'] if 'conv_f16s_kernel' in l['kernel'] and ', 0, ' in l['kernel'] and l['dur_ns'] >= 100e3]
-        if dom:
-            traffic = sum(l['dram_bytes'] for l in dom) / len(dom)
-            traffic_note = ('bytes per launch, dram__bytes_read.sum + dram__bytes_write.sum, mean over the %d dense conv_f16s launches of >= 100 us '
-                            'in the committed capture (%s: one eager B=1 forward, tools/ncu_ops.py; per-launch rows in profiles/r2_kernels_b1.md)'
-                            % (len(dom), tj['source']))
     achieved = conv_flops / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
 
     # ---- closed-loop latency (configs[1]): one frame per forward through the same model, graph replay
@@ -396,9 +423,9 @@ def main():
                      'mode': 'forward_inference(host batch): pinned-host inputs uploaded inside the call, ordered by first use and overlapped with the '
                              'kernels (LiDAR encoder under the image upload, key-frame images under the history sweeps), waypoints read back every step',
                      'phase_done_ms': e2e_trace},
-                roofline={'bound': 'tensor', 'kernel': 'conv_f16s_kernel (implicit-GEMM conv / linear / sparse-conv family on tcgen05, scaled-split fp16 operands; + the few SIMT fallbacks)',
+                roofline={'bound': 'tensor', 'kernel': 'conv_f16s_kernel (implicit-GEMM conv / linear / sparse-conv family on wgmma, scaled-split fp16 operands; + the few SIMT fallbacks)',
                           'achieved': achieved, 'peak': tensor_peak, 'unit': 'TFLOP/s', 'frac': achieved / tensor_peak,
-                          'traffic': traffic, 'traffic_note': traffic_note, 'peak_source': peak_src, 'launches_per_step': n_conv,
+                          'peak_source': peak_src, 'launches_per_step': n_conv,
                           'kernel_ms_per_step': conv_ms, 'kernel_share_of_step': conv_ms / eager_step_ms,
                           'share_note': 'per-launch CUDA events of one serial eager step (no graph, no stream overlap); share = '
                                         'family time / that step',

@@ -1,5 +1,5 @@
 /*
- * tt_b200.h — C ABI of libtt_b200.so: the B200-native (sm_100a) operator library for the
+ * tt_b200.h — C ABI of libtt_b200.so: the H100-native (sm_90a) operator library for the
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
  * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn).
@@ -36,8 +36,10 @@ int tt_version(void);
 const char* tt_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 long long tt_launch_count(void);
-/* diagnosis knobs for kernel micro-benchmarks (tools/conv_bench.py); 0 in normal operation */
-void tt_debug_set(int flags);
+/* diagnosis knobs for kernel micro-benchmarks (tools/conv_bench.py); 0 in normal operation.  128: no split-K in the tensor-core
+ * convs; bits 8..15: SMs the persistent tensor-core kernels leave free; 0x20000 / 0x40000: register accumulator folded every 4 / 1
+ * stages instead of 2; 0x200000: one tap per K slab in the output-stationary sparse conv.  Unknown bits: TT_ERR_INVALID, nothing set. */
+int tt_debug_set(int flags);
 
 /* ------------------------------------------------------------------------------------------
  * (1) voxel pooling — drop-in for the reference's only in-tree native op.
@@ -88,13 +90,13 @@ int tt_lift_splat(const tt_lift_splat_desc* d, const float* depth_logits, const 
  *   A[m][k], k = tap * Cin_g + c : the input pixel of output row m under tap (kh, kw), channel
  *   g*Cin_g + c, zero outside the image; or, when gather != NULL, row gather[m*taps + tap] of x
  *   (-1 = zero row) — the sparse-conv rulebook.
- *   w: impl 0/1: packed [taps * Cin_g][Cout] fp32 (BatchNorm already folded in); impl 2/3 (tcgen05): packed
+ *   w: impl 0/1: packed [taps * Cin_g][Cout] fp32 (BatchNorm already folded in); impl 2/3 (tensor cores): packed
  *      [2][Cout][taps][Cin] = `hi = RN_tf32(w)` plane followed by the `lo = RN_tf32(w - hi)` plane.  bias [Cout] or NULL.
  * Output row m = (n, oh, ow) is stored at pixel (n, oh*oy_mul + oy_add, ow*ox_mul + ox_add) of a
  * [N][yH][yW][y_ld] buffer (a k2s2 transposed conv is four such calls).
  * If m_count != NULL only the first *m_count rows (a device int) are computed.
- * `impl`: 0/1 = SIMT fp32 FFMA (exact), 2 = tcgen05 single-pass TF32 (operands rounded to nearest TF32),
- *         3 = tcgen05 3xTF32 (hi*hi + hi*lo + lo*hi, fp32-class); 4 = scaled-split fp16 through tt_conv2d_f16s.  impl 2/3 need stride 1 or 2, groups 1, channels,
+ * `impl`: 0/1 = SIMT fp32 FFMA (exact), 2 = tensor-core single-pass TF32 (operands rounded to nearest TF32),
+ *         3 = tensor-core 3xTF32 (hi*hi + hi*lo + lo*hi, fp32-class); 4 = scaled-split fp16 through tt_conv2d_f16s.  impl 2/3 need stride 1 or 2, groups 1, channels,
  *         x_ld, x_coff % 4 == 0 and 16-byte aligned x / w / y (TMA reads the activations in place and splits them in
  *         shared memory; no workspace); else TT_ERR_UNSUPPORTED.
  *         For impl 0/1 the workspace is optional: when given (size from tt_conv2d_workspace_bytes) small-M / large-K
@@ -251,7 +253,7 @@ int tt_sparse_rulebook(const tt_rulebook_desc* d, const int* in_coords, const in
  * launch walks every (tap, pair tile) and accumulates into the bias-initialised output rows with red.add.f32 (the
  * summation order across taps is not fixed: results repeat to fp32 rounding, not bitwise).
  * impl 0/1: SIMT fp32, w = [kvol][Cin][Cout] fp32 (BatchNorm folded).
- * impl 2/3: tcgen05 TF32 / 3xTF32 gather-GEMM, w = [2][Cout][kvol][Cin] hi / lo planes (as tt_conv2d); needs
+ * impl 2/3: tensor-core TF32 / 3xTF32 gather-GEMM, w = [2][Cout][kvol][Cin] hi / lo planes (as tt_conv2d); needs
  *           Cin, Cout >= 32 and % 4 == 0, in_ld / out_ld % 4 == 0, 16-byte aligned pointers, else TT_ERR_UNSUPPORTED.
  * res: optional [cap_out][res_ld] (SparseBasicBlock identity). */
 typedef struct {
@@ -271,7 +273,7 @@ int tt_sparse_conv_f16s(const tt_sparse_conv_desc* d, const void* feats_in_split
                         const int* out_count, float* feats_out, void* out_split, long long out_plane, tt_stream_t stream);
 /* Output-stationary sparse convolution on scaled-split fp16 operands: ONE launch, no atomics.  A work item is a tile of 128 output
  * rows; K runs over all kvol taps through the neighbour table `nbr` [cap_out][kvol] (input row under each tap, -1 = none: a zero
- * row), so the sum of an output row is formed in TMEM in a fixed order and stored once with bias + residual + activation fused
+ * row), so the sum of an output row is formed on the tensor cores in a fixed order and stored once with bias + residual + activation fused
  * (fp32 rows `io->y` and / or split planes `io->y_split`; residual as fp32 `io->res` or planes `io->res_split`).  Pays for empty
  * (row, tap) slots with zero rows — the better form once a fair share of the taps is populated (dilated / dense-ish clouds);
  * tt_sparse_conv_f16s (tap-major pair lists, red.add) is the form for very sparse neighbourhoods.  io->x_split = input planes

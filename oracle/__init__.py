@@ -8,7 +8,7 @@ the timed CPU baseline — never as the shipped path.
 What it is: a plain-PyTorch fp32 restatement of the reference forward
 (``/root/reference/open_loop_training``), module for module, with the same
 ``state_dict`` key names as the reference so that one set of weights drives both
-the oracle and the B200 path.  The reference itself cannot be imported in this
+the oracle and the H100 path.  The reference itself cannot be imported in this
 image (mmcv / mmdet / mmdet3d / spconv are absent), so third-party pieces
 (mmdet ResNet/PAFPN/BasicBlock, mmcv DCN / Voxelization / MSDA, mmdet3d
 HardSimpleVFE / SparseEncoder / SECOND / SECONDFPN, spconv) are restated from

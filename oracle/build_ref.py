@@ -19,11 +19,11 @@ def build(force=False):
         if os.path.exists(OUT):
             return OUT
         raise FileNotFoundError(SRC)
-    if os.path.exists(OUT) and not force and os.path.getmtime(OUT) >= os.path.getmtime(SRC):
+    if os.path.exists(OUT) and not force and os.path.getmtime(OUT) >= max(os.path.getmtime(SRC), os.path.getmtime(__file__)):   # (flags live here)
         return OUT
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     nvcc = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-    subprocess.check_call([nvcc, '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-shared', '-Xcompiler', '-fPIC',
+    subprocess.check_call([nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-shared', '-Xcompiler', '-fPIC',
                            '-o', OUT, SRC])
     return OUT
 

@@ -102,7 +102,7 @@ class Emu:
         return self.launches
 
     def tt_debug_set(self, flags):
-        pass
+        return 0
 
     def __getattr__(self, name):
         if name.endswith('_workspace_bytes'):

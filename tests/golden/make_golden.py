@@ -2,7 +2,7 @@
 
 The reference ships no tests or fixtures (SURVEY.md §4), so these vectors are produced by the oracle
 (oracle/ = plain-PyTorch restatement of the reference).  They pin (a) the oracle against accidental edits and
-(b) the B200 path against a stored answer that does not depend on re-running the oracle.  The end-to-end vectors are
+(b) the H100 path against a stored answer that does not depend on re-running the oracle.  The end-to-end vectors are
 re-derived with the reference's OWN code (same weights loaded into the reference EncoderDecoder behind import stubs) by
 tests/test_reference_golden_cpu.py::test_committed_plumbing_golden_is_reproduced_by_the_reference_code; vectors made
 directly by the reference's code live beside them as ref_*.npz (make_reference_golden.py).

@@ -218,12 +218,86 @@ def e2e_case(fw, regs):
     regs['BACKBONES'].classes['LidarNet'] = regs['stub_encoder']
 
 
+def calibrated_case(fw, regs):
+    """the reference's EncoderDecoder.forward_inference (its framework, LSS and decoder; LiDAR encoder = oracle stand-in) with the
+    oracle's seeded, BatchNorm-calibrated weights: the plumbing config at seeds 0..2 (the weights of tests/golden/plumbing_seed*.npz)
+    and the full thinktwice.py config at seed 0 (the bench workload, B = 1)."""
+    from oracle.lidar import LidarNet
+    from oracle.model import EncoderDecoder as Oracle, calibrate_bn, init_oracle_weights
+    from thinktwice_b200.config import Config, DEFAULT_CONFIG, PLUMBING_CONFIG
+    from thinktwice_b200.synthetic import make_batch
+    lss = sys.modules['olt_code.model_code.backbones.lss']
+    regs['BACKBONES'].classes['LSS'], regs['BACKBONES'].classes['LidarNet'] = lss.LSS, LidarNet
+    for name, path, seeds, points in (('plumbing', PLUMBING_CONFIG, (0, 1, 2), 2000), ('full', DEFAULT_CONFIG, (0,), 40000)):
+        mc = Config.fromfile(path).model
+        for seed in seeds:
+            o = Oracle(**{k: v for k, v in mc.items() if k != 'type'})
+            init_oracle_weights(o, seed)
+            batch = make_batch(Config.fromfile(path), 1, seed=seed, num_points=points)
+            calibrate_bn(o, batch)
+            ref = fw.EncoderDecoder(img_encoder=dict(mc['img_encoder']), decoder=dict(mc['decoder']), lidar_encoder=dict(mc['lidar_encoder']),
+                                    train_cfg=mc['train_cfg'], test_cfg=mc.get('test_cfg')).eval()
+            ref.load_state_dict(o.state_dict())
+            batch['target_command_raw'] = batch['target_command'].argmax(-1)
+            with torch.no_grad():
+                pred = ref.forward_inference(batch)
+            keys = PRED_KEYS if name == 'full' else PRED_KEYS[:-1]
+            np.savez_compressed(os.path.join(HERE, f'ref_calibrated_{name}_seed{seed}.npz'), **{k: pred[k].detach().cpu().numpy() for k in keys})
+            print(f'calibrated {name} seed {seed}: pred_wp[-1] = {[round(float(v), 4) for v in pred["pred_wp"][0, -1].flatten()]}')
+    regs['BACKBONES'].classes['LSS'] = regs['stub_encoder']
+    regs['BACKBONES'].classes['LidarNet'] = regs['stub_encoder']
+
+
+GEOM_SAMPLE = 8192
+
+
+def camera_geometry_case(regs):
+    """what the reference LSS computes on the host side of the camera branch, for the plumbing and the full config (B = 2, batch
+    seed 3): create_frustum, the voxel grid constants, get_geometry per sweep (on the matrices LSS.forward assembles; a seeded sample of
+    GEOM_SAMPLE points and their integer voxel indices) and the 22-wide tensor DepthNet feeds its BatchNorm1d."""
+    from thinktwice_b200.config import Config, DEFAULT_CONFIG, PLUMBING_CONFIG
+    from thinktwice_b200.registry import BACKBONES
+    from thinktwice_b200.synthetic import make_batch
+    lss = sys.modules['olt_code.model_code.backbones.lss']
+    for which, path in (('plumbing', PLUMBING_CONFIG), ('full', DEFAULT_CONFIG)):
+        cfg = Config.fromfile(path)
+        kw = {k: v for k, v in dict(cfg.model['img_encoder']).items() if k != 'type'}
+        ref = lss.LSS(**kw).eval()
+        prod = BACKBONES.build(dict(cfg.model['img_encoder']))          # (only its build_mats: the matrices LSS.forward assembles)
+        B = 2
+        batch = make_batch(cfg, B, seed=3, num_points=10)
+        metas = batch['img_metas']
+        N = batch['img'].shape[2]
+        mats = prod.build_mats(metas, N)
+        out = dict(frustum=ref.frustum.numpy(), lower=(ref.voxel_coord - ref.voxel_size / 2.0).numpy(), voxel_size=ref.voxel_size.numpy(),
+                   voxel_num=np.array([int(v) for v in ref.voxel_num]))
+        lower = ref.voxel_coord - ref.voxel_size / 2.0
+        for s in range(len(metas[0])):
+            idx = -1 if s == 0 else -s                                  # the sweep index LSS.forward passes (lss.py:689, 712)
+            geom = ref.get_geometry(mats['sensor2ego_mats'][:, idx], mats['intrin_mats'][:, idx], mats['ida_mats'][:, idx], None)
+            flat = geom.reshape(-1, 3)
+            pos = torch.randperm(flat.shape[0], generator=torch.Generator().manual_seed(s))[:GEOM_SAMPLE].sort().values
+            out[f'geom{s}_pos'] = pos.numpy()
+            out[f'geom{s}'] = flat[pos].numpy()
+            out[f'geom{s}_voxel'] = ((flat[pos] - lower) / ref.voxel_size).int().numpy()
+        seen = {}
+        h = ref.depth_net.bn.register_forward_pre_hook(lambda m, inp: seen.setdefault('x', inp[0].detach().clone()))
+        with torch.no_grad():
+            ref.depth_net(torch.zeros(B * N, kw['depth_net_conf']['in_channels'], 2, 2), {k: v for k, v in mats.items()})
+        h.remove()
+        out['depthnet_bn_input'] = seen['x'].reshape(B * N, 22).numpy()
+        np.savez_compressed(os.path.join(HERE, f'ref_camera_geometry_{which}.npz'), **out)
+        print(f'camera geometry {which}: frustum {tuple(ref.frustum.shape)}, {len(metas[0])} sweeps')
+
+
 def main():
     from thinktwice_b200.config import Config, DEFAULT_CONFIG
     cfg = Config.fromfile(DEFAULT_CONFIG)
     fw, regs = load_reference()
     lss_case(regs)
     e2e_case(fw, regs)
+    calibrated_case(fw, regs)
+    camera_geometry_case(regs)
     mc = cfg.model
     regs['BACKBONES'].classes['LSS'] = regs['stub_encoder']            # (importing lss.py registered the real LSS)
     for seed, B in ((0, 1), (1, 1), (2, 2)):                           # B = 2: the Look module couples the frames of a batch (SURVEY fact 4)

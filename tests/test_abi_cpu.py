@@ -58,13 +58,12 @@ def test_product_fails_loudly_without_cuda():
 
 
 def test_config_model_section_equals_reference_when_present():
+    """the `model` section of the reference's configs/thinktwice.py, stored as tests/golden/ref_thinktwice_config_model.json"""
+    import json
     from thinktwice_b200.config import Config, DEFAULT_CONFIG
-    ref_path = '/root/reference/open_loop_training/configs/thinktwice.py'
     ours = Config.fromfile(DEFAULT_CONFIG)
     assert ours.model.decoder.config.pred_len == 4 and ours.model.img_encoder.final_dim == (448, 896)
-    if not os.path.exists(ref_path):
-        return
-    ref = Config.fromfile(ref_path)
+    ref = json.load(open(os.path.join(ROOT, 'tests', 'golden', 'ref_thinktwice_config_model.json')))
 
     def norm(x):
         if isinstance(x, dict):
@@ -81,7 +80,7 @@ def test_config_model_section_equals_reference_when_present():
         elif a != b:
             out.append((path, a, b))
         return out
-    assert not diff(norm(ours.model), norm(ref.model))
+    assert not diff(norm(ours.model), ref)
 
 
 def test_ctypes_structs_match_the_c_header(tmp_path):

@@ -1,4 +1,4 @@
-"""tcgen05 convolution on scaled-split fp16 operands (csrc/gemm_conv_f16s.cu, impl 4) against an fp64 torch reference.
+"""Tensor-core (wgmma) convolution on scaled-split fp16 operands (csrc/gemm_conv_f16s.cu, impl 4) against an fp64 torch reference.
 Same case list as the 3xTF32 kernel (tests/test_tc_gpu.py): the two engines share the tiling and the epilogue contract.
 Every case also checks the split planes the epilogue writes (hi + lo'/2048 == the fp32 output to 2^-22)."""
 import ctypes as C

@@ -1,4 +1,4 @@
-"""GPU: the B200 path reproduces the committed golden vectors (end-to-end plumbing config + per-op cases)."""
+"""GPU: the H100 path reproduces the committed golden vectors (end-to-end plumbing config + per-op cases)."""
 import ctypes as C
 import os
 

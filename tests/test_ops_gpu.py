@@ -190,10 +190,26 @@ def test_voxel_pooling_dropin_matches_oracle_and_reference_kernel(shape):
     out = voxel_pooling(geom.cuda().contiguous(), feats.cuda().contiguous(), vn.cuda())
     assert out.shape == (B, Cc, Y, X)
     assert relerr(out, ref) < 1e-5
-    # the reference's own kernel, compiled from /root/reference into oracle/_ref (same box, same inputs)
+    from thinktwice_b200.ops.voxel_pooling import last_pos_memo
+    # the reference's own kernel: compiled into oracle/_ref by build() where the reference sources are present (same box, same
+    # inputs); otherwise what it returned for these inputs, stored by tests/golden/make_voxel_pool_golden.py
     so = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle', '_ref', 'libvoxel_pooling_ref.so')
     if not os.path.exists(so):
-        pytest.skip('oracle/_ref not built (reference sources absent at build time)')
+        gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_voxel_pool_%d_%d_%d_%d_%d.npz' % shape))
+        pos, rows = torch.from_numpy(gold['out_pos']).long(), torch.from_numpy(gold['memo_rows']).long()
+        assert relerr(out.reshape(-1).cpu()[pos], torch.from_numpy(gold['out'])) < 1e-5
+        assert torch.equal(last_pos_memo().reshape(B * P, 3).cpu()[rows], torch.from_numpy(gold['memo']))
+        from thinktwice_b200 import lib as ttlib                      # the link-level drop-in symbol of libtt_b200.so
+        fn3 = getattr(C.CDLL(ttlib.LIB_PATH), '_Z37voxel_pooling_forward_kernel_launcheriiiiiiPKiPKfPfPiP11CUstream_st')
+        g, f = geom.cuda().contiguous(), feats.cuda().contiguous()
+        o3 = torch.zeros(B, Y, X, Cc, device='cuda')
+        memo3 = -torch.ones(B, P, 3, dtype=torch.int32, device='cuda')
+        fn3(B, P, Cc, X, Y, 1, C.c_void_p(g.data_ptr()), C.c_void_p(f.data_ptr()), C.c_void_p(o3.data_ptr()),
+            C.c_void_p(memo3.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        torch.cuda.synchronize()
+        assert relerr(o3.permute(0, 3, 1, 2).reshape(-1).cpu()[pos], torch.from_numpy(gold['out'])) < 1e-5
+        assert torch.equal(memo3.reshape(B * P, 3).cpu()[rows], torch.from_numpy(gold['memo']))
+        return
     lib = C.CDLL(so)
     fn = getattr(lib, '_Z37voxel_pooling_forward_kernel_launcheriiiiiiPKiPKfPfPiP11CUstream_st')
     g, f = geom.cuda().contiguous(), feats.cuda().contiguous()
@@ -203,7 +219,6 @@ def test_voxel_pooling_dropin_matches_oracle_and_reference_kernel(shape):
        C.c_void_p(memo.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
     assert relerr(out, o2.permute(0, 3, 1, 2)) < 1e-5
-    from thinktwice_b200.ops.voxel_pooling import last_pos_memo
     assert torch.equal(last_pos_memo(), memo)                     # integer side: bit-exact
     # the product's link-level drop-in: the SAME mangled symbol exported by libtt_b200.so (voxel_pooling_forward.cpp:21-22)
     from thinktwice_b200 import lib as ttlib
@@ -323,7 +338,7 @@ def test_voxelize_mean_matches_oracle(eng):
 
 @pytest.mark.parametrize('Cin,Cout,density,impl', [(16, 32, 0.08, 1), (64, 128, 0.25, 3), (32, 32, 0.3, 3), (128, 64, 0.15, 3)])
 def test_sparse_conv_layers_match_oracle(Cin, Cout, density, impl):
-    """impl 1: fused SIMT gather GEMM; impl 3: tcgen05 3xTF32 gather GEMM (cp.async row gather, red.add epilogue)."""
+    """impl 1: fused SIMT gather GEMM; impl 3: tensor-core 3xTF32 gather GEMM (cp.async row gather, red.add epilogue)."""
     from oracle.lidar import SparseConvBase, SparseTensor
     from thinktwice_b200.lib import RulebookDesc, _p
     from thinktwice_b200 import lib

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution (TMA + TMEM, 3xTF32 / single-pass TF32) against an fp64 torch reference."""
+"""wgmma implicit-GEMM convolution (TMA + register accumulators, 3xTF32 / single-pass TF32) against an fp64 torch reference."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -61,7 +61,7 @@ def test_tc_conv_matches_fp64(case, impl, tol):
     n0 = lib.launch_count()
     y = eng.conv(to_fmap(x.cuda()), pw, name='tc.y', stride=stride, pad=p, dil=dil, act=act)
     torch.cuda.synchronize()
-    assert 1 <= lib.launch_count() - n0 <= 3       # one tcgen05 kernel (+ split-K init / activation passes)
+    assert 1 <= lib.launch_count() - n0 <= 3       # one tensor-core kernel (+ split-K init / activation passes)
     ref = F.conv2d(x.double(), w.double(), b.double() if bias else None, stride=stride, padding=p, dilation=dil)
     ref = {0: ref, 1: F.relu(ref), 2: F.gelu(ref), 3: torch.sigmoid(ref)}[act]
     err = relerr(y.nchw(), ref)
@@ -127,7 +127,7 @@ def test_tc_split_k_for_underfilled_layers(case):
     n0 = lib.launch_count()
     y = eng.conv(to_fmap(x.cuda()), pw, name='tc.sk', pad=p, act=act, res=to_fmap(r.cuda()) if use_res else None)
     torch.cuda.synchronize()
-    assert lib.launch_count() - n0 == (3 if act else 2)          # init + split-K tcgen05 kernel (+ activation pass)
+    assert lib.launch_count() - n0 == (3 if act else 2)          # init + split-K tensor-core kernel (+ activation pass)
     ref = F.conv2d(x.double(), w.double(), sd['c.bias'].double() if bias else None, padding=p)
     if use_res:
         ref = ref + r.double()
@@ -138,7 +138,7 @@ def test_tc_split_k_for_underfilled_layers(case):
 @pytest.mark.parametrize('impl,tol', [(1, 2e-6), (3, 3e-6)])
 def test_rowpacked_stem_conv_matches_fp64(impl, tol):
     """7x7 s2 p3 conv on 3 channels as a 7x1 conv over 32 row-packed "channels" of a zero-bordered channels-last image
-    (tt_conv_desc.x_hstride, x_ld < Cin): SIMT and tcgen05 against torch fp64."""
+    (tt_conv_desc.x_hstride, x_ld < Cin): SIMT and tensor cores against torch fp64."""
     from thinktwice_b200 import lib
     from thinktwice_b200.engine import Engine, FMap
     from thinktwice_b200.weights import Packer

@@ -1,4 +1,4 @@
-"""thinktwice_b200 — B200-native implementation of the ThinkTwice per-frame forward path.
+"""thinktwice_b200 — H100-native implementation of the ThinkTwice per-frame forward path.
 
 Importing the package registers the boundary classes (EncoderDecoder, LSS, LidarNet, SparseEncoder_fp32,
 ThinkTwiceDecoder) exactly like the reference's plugin import does (open_loop_training/code/__init__.py).

@@ -1,4 +1,4 @@
-"""In-tree build of libtt_b200.so (nvcc, sm_100a only).  Used by __graft_entry__.build()."""
+"""In-tree build of libtt_b200.so (nvcc, sm_90a only).  Used by __graft_entry__.build()."""
 import glob
 import hashlib
 import os
@@ -7,7 +7,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libtt_b200.so')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 
@@ -40,7 +40,7 @@ def build(force=False, verbose=False):
             print(' '.join(cmd)); print(out)
         if p.returncode:
             raise RuntimeError('nvcc failed: ' + ' '.join(cmd))
-    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB] + objs
+    cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB] + objs
     subprocess.check_call(cmd)
     with open(stamp, 'w') as f:
         f.write(dig)

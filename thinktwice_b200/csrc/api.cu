@@ -26,7 +26,16 @@ extern "C" {
 int tt_version(void) { return 100; }
 const char* tt_last_error(void) { return g_err; }
 long long tt_launch_count(void) { return g_tt_launches; }
-void tt_debug_set(int flags) { g_tt_debug = flags; }
+int tt_debug_set(int flags) {
+  // the knobs the kernels read (include/tt_b200.h); anything else is refused so that no experiment silently measures the default path
+  const int known = 128 | 0xFF00 | 0x20000 | 0x40000 | 0x200000;
+  if (flags & ~known) {
+    tt_set_error("tt_debug_set: unknown knob bits 0x%x", flags & ~known);
+    return TT_ERR_INVALID;
+  }
+  g_tt_debug = flags;
+  return TT_OK;
+}
 
 int tt_conv2d(const tt_conv_desc* d, const float* x, const float* w, const float* bias, const float* res,
               const float* res2, const int* gather, const int* m_count, float* y, void* workspace, tt_stream_t stream) {
@@ -39,7 +48,7 @@ int tt_conv2d(const tt_conv_desc* d, const float* x, const float* w, const float
   if (impl >= 2) {
     if (gather || m_count || !tt_conv2d_tc_supported(d, x, w, y) || ((reinterpret_cast<uintptr_t>(res) | reinterpret_cast<uintptr_t>(res2) |
                                                                        reinterpret_cast<uintptr_t>(bias)) & 15)) {
-      tt_set_error("tt_conv2d: tcgen05 path does not support this shape / alignment");
+      tt_set_error("tt_conv2d: tensor-core path does not support this shape / alignment");
       return TT_ERR_UNSUPPORTED;
     }
     return tt_conv2d_tc(d, x, w, bias, res, res2, y, workspace, st);

@@ -163,11 +163,11 @@ int tt_voxel_pooling_backward(int batch_size, int num_points, int num_channels, 
                     (stride_c != 1 || ((reinterpret_cast<uintptr_t>(grad_output) & 15) == 0 && ((stride_b | stride_y | stride_x) & 3) == 0));
   if (vec4) {
     const long long total4 = total / 4, want4 = (total4 + 255) / 256;
-    voxel_pool_bwd4_kernel<<<(int)(want4 > 148 * 32 ? 148 * 32 : want4), 256, 0, (cudaStream_t)stream>>>(
+    voxel_pool_bwd4_kernel<<<(int)(want4 > tt_num_sms() * 32 ? tt_num_sms() * 32 : want4), 256, 0, (cudaStream_t)stream>>>(
         grad_output, stride_b, stride_c, stride_y, stride_x, pos_memo, reinterpret_cast<float4*>(grad_input), total4, num_channels / 4);
   } else {
     const long long want = (total + 255) / 256;
-    voxel_pool_bwd_kernel<<<(int)(want > 148 * 32 ? 148 * 32 : want), 256, 0, (cudaStream_t)stream>>>(grad_output, stride_b, stride_c, stride_y, stride_x,
+    voxel_pool_bwd_kernel<<<(int)(want > tt_num_sms() * 32 ? tt_num_sms() * 32 : want), 256, 0, (cudaStream_t)stream>>>(grad_output, stride_b, stride_c, stride_y, stride_x,
                                                                                                       pos_memo, grad_input, total, num_channels);
   }
   ++g_tt_launches;

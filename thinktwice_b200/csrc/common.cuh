@@ -1,4 +1,4 @@
-// Shared helpers for the tt_b200 kernels (sm_100a only).
+// Shared helpers for the tt_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,10 +31,16 @@ void tt_set_error(const char* fmt, ...);
 
 static inline int tt_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// SM count of the current device (cached): the CTA count of the persistent kernels and the grid cap of the grid-stride ones
+static inline int tt_num_sms() {
+  static int n = 0;
+  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); }
+  return n;
+}
+
 // Activations.  NONE / RELU are inlined; everything with a transcendental (erff, expf, log1pf are ~100 SASS
 // instructions each) lives in ONE out-of-line copy per translation unit: inlining it into fully unrolled GEMM
-// epilogues blew the tcgen05 kernel up to 392 KB of SASS and made its epilogue instruction-cache bound
-// (profiles/r1_summary_tc.md).
+// epilogues blows a tensor-core kernel up by hundreds of KB of SASS and makes its epilogue instruction-cache bound.
 static __device__ __noinline__ float tt_act_slow(float v, int act) {
   switch (act) {
     case TT_ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752440f));

@@ -53,7 +53,7 @@ extern "C" int tt_dcn_im2col(const float* x, const float* offset, int off_ld, fl
   const long long total = (long long)N * H * W * 9 * (C / 4);
   if (total == 0) return TT_OK;
   const long long nb = (total + 255) / 256;
-  dcn_im2col_kernel<<<(int)(nb > 148 * 32 ? 148 * 32 : nb), 256, 0, (cudaStream_t)stream>>>(x, offset, off_ld, col, N, H, W,
+  dcn_im2col_kernel<<<(int)(nb > tt_num_sms() * 32 ? tt_num_sms() * 32 : nb), 256, 0, (cudaStream_t)stream>>>(x, offset, off_ld, col, N, H, W,
                                                                                          C, groups, total);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_dcn_im2col");

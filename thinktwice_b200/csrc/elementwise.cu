@@ -9,7 +9,7 @@ extern long long g_tt_launches;
 namespace {
 
 constexpr int TPB = 256;
-inline int blocks_for(long long n, int cap = 148 * 16) {
+inline int blocks_for(long long n, int cap = tt_num_sms() * 16) {
   long long b = (n + TPB - 1) / TPB;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }

@@ -1,24 +1,24 @@
-// tcgen05 implicit-GEMM convolution on SCALED-SPLIT FP16 operands ("f16s") for sm_100a — the round-2 successor of the
-// 3xTF32 kernel in gemm_conv_tc.cu (same tiling, same epilogue contract, same fp32-class accuracy, half the operand bytes
-// and twice the tensor-core rate).
+// Hopper (sm_90a) implicit-GEMM convolution on SCALED-SPLIT FP16 operands ("f16s") — the successor of the 3xTF32 kernel in
+// gemm_conv_tc.cu (same tiling, same epilogue contract, same fp32-class accuracy, half the operand bytes and twice the
+// tensor-core rate).
 //
 // Operand format.  An fp32 value x is carried as two halves:  hi = RN_f16(x),  lo = RN_f16((x - hi) * 2^11).
 //   x - hi is exact in fp32 and |x - hi| <= 2^-11 |x|, so lo is O(|x|) again (no fp16 underflow of the correction) and
 //   x = hi + lo * 2^-11 to 2^-22 relative (fp16 has the same 11 significant bits as TF32): the same representation error as
 //   the TF32 hi / lo split, at 4 bytes per element instead of 8.  Activations live in HBM in this form next to (or instead
 //   of) their fp32 copy: a "split" tensor is two half planes [2][N][H][W][ld] written by the PRODUCING kernel's epilogue, so
-//   the consumer's TMA loads deliver tensor-core-ready operands — no split warps, no shared-memory rewrite (the 3xTF32
-//   kernel's measured roof was shared-memory traffic: 176 KB per 32-float K slab, profiles/r1_tc_full_summary.md).
+//   the consumer's TMA loads deliver tensor-core-ready operands — no split pass, no shared-memory rewrite.
 //   Range: |x| must stay below 65504 (hi saturates; counted in g_f16s_saturated, read with tt_f16s_saturation_count).
-// Products.  Per K step (16 halves) two instructions, exactly the 3-product scheme of the TF32 kernel:
-//   main | corr  +=  A_hi x [B_hi ; B_lo']      one N = 2 BN tcgen05.mma.kind::f16 (B_lo' follows B_hi in shared memory)
-//   corr         +=  A_lo' x B_hi
-//   result = main + 2^-11 corr  (the dropped lo x lo term is 2^-22 relative).  kind::f16 K = 16 per instruction, so a K of
-//   128 costs the 8 truncating accumulations that 64 cost in TF32: chunks (TMEM ping-pong drains into fp32 registers, see
-//   gemm_conv_tc.cu) are twice as long at the same accumulated rounding error.
-// Everything else follows gemm_conv_tc.cu: TMA box loads per tap (zero fill = padding, element strides = stride 2), CTA pairs
-// with multicast weight halves, persistent tiles, 8 epilogue warps with coalesced stores, split-K and GATHER (sparse conv).
-// Warp roles: warp 0 = TMA / gather producer, warp 1 = TMEM allocator + MMA issuer, warps 2..9 = epilogue.
+// Products.  Per K step (16 halves) three m64nBNk16 wgmma per warpgroup, the 3-product scheme of the TF32 kernel:
+//   main  +=  A_hi x B_hi,   corr  +=  A_hi x B_lo',   corr  +=  A_lo' x B_hi
+//   result = main + 2^-11 corr  (the dropped lo x lo term is 2^-22 relative).  main and corr are separate register arrays and every
+//   instruction has the same shape: wgmma of different shapes on overlapping accumulators would be serialised by the compiler.  The register accumulator is restarted every
+//   `chunk` stages and folded into fp32 sums with round-to-nearest FMAs, so the tensor core's own accumulation only ever
+//   spans 2 x 64 K elements.
+// Tiling follows gemm_conv_tc.cu: TMA box loads per tap (zero fill = padding, element strides = stride 2), persistent CTAs
+// (one per SM), split-K and GATHER (sparse convolution).
+// Warp roles: warpgroup 0 = producer (warp 0: TMA / gather; warps 1..3 idle);
+// warpgroups 1 and 2 = wgmma + epilogue for rows 0..63 / 64..127 of the tile.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -33,81 +33,19 @@ __device__ unsigned int g_f16s_saturated = 0;     // number of values an epilogu
 
 namespace {
 
-constexpr int BM = 128;           // UMMA M
+constexpr int BM = 128;           // M tile: two warpgroups x 64 rows
 constexpr int KE = 64;            // K elements per stage (one 128-byte swizzle row of halves)
-constexpr int NTHREADS = 320;     // warp 0 producer, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
+constexpr int NTHREADS = 384;     // warpgroup 0 producer, warpgroups 1..2 MMA + epilogue
 constexpr float LO_SCALE = 2048.f, LO_INV = 1.f / 2048.f;
 constexpr int MAX_KVOL = 32;
 constexpr float H_MAX = 65504.f;
 
-// kind::f16 instruction descriptor: c_format F32 (1) @4, a/b_format F16 (0) @7/@10, K-major, N >> 3 @17, M >> 4 @24
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-TT_DEVICE void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 TT_DEVICE void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
   asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(
           smem_u32(dst)),
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
-}
-TT_DEVICE void tma_load_4d_mc(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(mask)
-      : "memory");
-}
-
-
-// ---- cta_group::2 (CTA-pair MMA): one instruction of the pair's leader drives both SMs' tensor cores over M = 256 (128 rows from each
-// CTA's own shared memory) and an N whose B rows are split between the two CTAs — each SM reads its A tile and only HALF of B.
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;   // shared::cluster address of the same offset in the pair's even-ranked CTA (cute: Sm100MmaPeerBitMask)
-TT_DEVICE void umma_f16_2cta(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-// completion of every tcgen05 operation this thread issued so far -> the barrier at this offset in BOTH CTAs of the pair
-TT_DEVICE void tcgen05_commit_2cta(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// TMA loads into this CTA's shared memory that signal the LEADER's mbarrier (the pair's MMA issuer waits on one barrier for both CTAs' operands)
-TT_DEVICE void tma2_load_3d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-TT_DEVICE void tma2_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-TT_DEVICE void tma2_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(
-          smem_u32(dst)),
-      "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-// one arrival on the barrier at this offset in the pair's leader CTA (a plain local arrive when executed by the leader itself)
-TT_DEVICE void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_MASK) : "memory");
 }
 
 // x -> (hi, lo') with saturation to the fp16 range; returns true when x had to be clamped
@@ -153,9 +91,8 @@ struct HArgs {
   int tiles_w, tiles_h;
   int flat;
   int n_slabs;           // ceil(Cin / 64)
-  int chunk;             // stages accumulated inside TMEM before the epilogue folds them into fp32 registers
+  int chunk;             // stages accumulated by the tensor core before the epilogue warpgroups fold them into fp32 sums
   int total_pix;
-  int dbg;
   int m_tiles, n_tiles;
   // GATHER (tap-major sparse convolution)
   const __half* gx;      // split feature rows: hi plane [.][gx_ld], lo' plane gx_plane halves further
@@ -170,42 +107,26 @@ struct HArgs {
   int cap_rows;
   int tps;               // output-stationary: taps per 64-half K slab (2 when Cin == 32, else 1)
   int splits, k_per;     // split-K: K stages per split
-  int corr_once;         // correction accumulator kept in TMEM for the whole K walk of a work item and drained once (see the MMA issuer)
 };
 
 // GM (gather mode): 0 = dense convolution (TMA box loads); 1 = tap-major sparse convolution (work item = one tap's pair tile,
 // red.add epilogue); 2 = output-stationary sparse convolution (work item = an output-row tile, K runs over ALL taps through the
 // neighbour table, plain fused epilogue — no atomics, no init / finish passes; pays for empty (row, tap) slots with zero rows).
-template <int BN, int STAGES, int GM, bool PAIR, int EW, bool CO, int CG>
-__global__ void __launch_bounds__(64 + 32 * EW, 1)
+template <int BN, int STAGES, int GM>
+__global__ void __launch_bounds__(NTHREADS, 1)
 conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const HArgs p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   constexpr int A_BYTES = BM * KE * 2;                    // 16 KB per plane
   constexpr int B_BYTES = BN * KE * 2;                    // per plane
-  // CG == 2 (cta_group::2): the stage holds this CTA's A planes, ONE 128-row weight block (the hi plane in the leader, the lo' plane in
-  // its peer: together the N = 2 BN operand [B_hi ; B_lo'] of the combined instruction) and this CTA's half of B_hi for the lo' x hi product
-  static_assert(CG == 1 || (PAIR && GM == 0 && !CO), "cta_group::2 path: dense convolutions on CTA pairs only");
-  constexpr int STAGE_BYTES = CG == 2 ? 2 * A_BYTES + B_BYTES + B_BYTES / 2 : 2 * A_BYTES + 2 * B_BYTES;
-  constexpr int ACC_COLS = 2 * BN;                        // main | corr
-  constexpr int TMEM_COLS = 2 * ACC_COLS;                 // ping-pong
-  constexpr int SLAB = 16;
-  constexpr int PITCH = SLAB + 4;
-  constexpr int HN = BN / (EW / 4);                        // columns owned by one epilogue warp (EW / 4 warps per TMEM lane quarter)
-  constexpr int RPP = EW == 16 ? 16 : 32;                 // rows per transposition phase: the slab buffers stay 20 KB in total
+  constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+  constexpr int SLAB = 16;                                // epilogue column slab
+  constexpr int PITCH = SLAB + 4;                         // +4 floats: conflict-free transposition
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* tile_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);              // [8 warps][32 rows][PITCH]
-  long long* row_y = reinterpret_cast<long long*>(tile_all + 8 * 32 * PITCH);
-  long long* row_r1 = row_y + BM;
-  long long* row_r2 = row_r1 + BM;
-  int* row_flag = reinterpret_cast<int*>(row_r2 + BM);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(row_flag + BM);
+  float* tile_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);              // [8 MMA warps][16 rows][PITCH]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tile_all + 8 * 16 * PITCH);
   uint64_t* full = bars;                                  // [STAGES]  producer -> MMA (operands landed)
-  uint64_t* empty = bars + STAGES;                        // [STAGES]  MMA -> producer
-  uint64_t* acc_full = bars + 2 * STAGES;                 // [2]       MMA -> epilogue
-  uint64_t* acc_empty = bars + 2 * STAGES + 2;            // [2]       epilogue -> MMA
-  uint64_t* corr_empty = bars + 2 * STAGES + 4;           // [2]       epilogue -> MMA (corr_once: correction buffer of work item t & 1 drained)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 6);
-  int* sp_first = reinterpret_cast<int*>(tmem_slot + 2);
+  uint64_t* empty = bars + STAGES;                        // [STAGES]  MMA warps -> producer
+  int* sp_first = reinterpret_cast<int*>(bars + 2 * STAGES);
   int* sp_cnt = sp_first + MAX_KVOL + 1;
 
   const tt_conv_desc& d = p.d;
@@ -215,15 +136,9 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   // output-stationary with Cin = 32: a 64-half K slab holds TWO taps (p.tps = 2), so no half of a slab is padding
   const int k_iters = (GM == 2 && p.tps == 2) ? (p.kvol + 1) / 2 : taps * p.n_slabs;
   const int os_rows = GM == 2 ? min(*p.out_count, p.cap_rows) : 0;     // output-stationary: rows that exist (device count)
-  // PAIR: CTA pairs (cluster of 2) walk two M tiles of the same N tile in lockstep and multicast weight halves to each other;
-  // !PAIR: every CTA is on its own (loads the whole weight slab itself, no cross-CTA barriers) — measured alternative
-  constexpr int CL = PAIR ? 2 : 1;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int pair0 = blockIdx.x / CL, pair_step = gridDim.x / CL;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GATHER ? 33 : 1); mbar_init(&empty[s], CG == 2 ? 1 : CL); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], CG == 2 ? 2 * EW : EW); mbar_init(&corr_empty[b], EW); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GATHER ? 33 : 1); mbar_init(&empty[s], 8); }   // 8 MMA warps release a stage
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (GM == 1 && threadIdx.x == 64) {
@@ -232,26 +147,13 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       const int c = min(p.pair_count[t], p.pair_cap);
       sp_cnt[t] = c;
       sp_first[t] = acc;
-      acc += ((c + BM - 1) / BM + CL - 1) / CL;
+      acc += (c + BM - 1) / BM;
     }
     sp_first[p.kvol] = acc;
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) {                                  // the same columns in both CTAs of the pair (issued by both)
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  cluster_sync_all();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int os_tiles = (os_rows + BM - 1) / BM;
-  const int total_pairs = (GM == 1 ? sp_first[p.kvol] : ((GM == 2 ? os_tiles : p.m_tiles) + CL - 1) / CL) * p.n_tiles * p.splits;
+  const int total_items = (GM == 1 ? sp_first[p.kvol] : GM == 2 ? os_tiles : p.m_tiles) * p.n_tiles * p.splits;
   auto decode = [&](int pt, int& nt, int& mt, int& tap, int& count, int& kb, int& ke) {
     const int ks = pt % p.splits;
     pt /= p.splits;
@@ -261,147 +163,141 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     const int pm = pt / p.n_tiles;
     tap = 0; count = 0;
     if (GM == 2) {
-      mt = CL * pm + (int)rank;
+      mt = pm;
       count = os_rows;
     } else if (GM == 1) {
       while (sp_first[tap + 1] <= pm) ++tap;
-      mt = CL * (pm - sp_first[tap]) + (int)rank;
+      mt = pm - sp_first[tap];
       count = sp_cnt[tap];
     } else {
-      mt = CL * pm + (int)rank;
+      mt = pm;
     }
   };
 
-  // weight slab of one stage: hi plane then lo' plane, BN rows each.  PAIR: this CTA loads its half of each plane and multicasts
-  // it to both CTAs of the pair; !PAIR: it loads both halves for itself.
+  // weight slab of one stage: hi plane then lo' plane, BN rows each, loaded as two BN / 2-row boxes per plane
   auto load_weights = [&](uint8_t* st, uint64_t* bar, int k0, int tap, int n0) {
     uint8_t* bh = st + 2 * A_BYTES;
-    if (PAIR) {
-      tma_load_4d_mc(bh + rank * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + (int)rank * (BN / 2), 0, 3);
-      tma_load_4d_mc(bh + B_BYTES + rank * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + (int)rank * (BN / 2), 1, 3);
-    } else {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        tma_load_4d(bh + h * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + h * (BN / 2), 0);
-        tma_load_4d(bh + B_BYTES + h * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + h * (BN / 2), 1);
-      }
+    for (int h = 0; h < 2; ++h) {
+      tma_load_4d(bh + h * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + h * (BN / 2), 0);
+      tma_load_4d(bh + B_BYTES + h * (B_BYTES / 2), &map_b, bar, k0, tap, n0 + h * (BN / 2), 1);
     }
   };
 
-  if (warp == 0 && GATHER) {
-    // ===================================================================== gather producer (whole warp) + weight TMA
-    const uint32_t txb = 2 * B_BYTES;
-    int ig = 0;
-    for (int pt = pair0; pt < total_pairs; pt += pair_step) {
-      int nt, mt, tap, count, kb, ke;
-      decode(pt, nt, mt, tap, count, kb, ke);
-      const int n0 = nt * BN;
-      const int* pin = GM == 1 ? p.pairs_in + (long long)tap * p.pair_cap : nullptr;
-      int rows[4];
-      int nxa[4] = {-1, -1, -1, -1}, nxb[4] = {-1, -1, -1, -1};   // neighbour indices of the next stage / tap (GM == 2)
-      if (GM == 1) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int m = mt * BM + lane + 32 * i;
-          rows[i] = m < count ? __ldg(pin + m) : -1;
-        }
-      }
-      for (int it = kb; it < ke; ++it, ++ig) {
-        const int s = ig % STAGES;
-        if (GM == 2 && p.tps == 2) {
-          // ---- two taps per K slab (Cin = 32): chunks 0..3 of a row come from the neighbour under tap 2 it, chunks 4..7 from tap 2 it + 1
-          // (the neighbour indices of stage it + 1 are fetched while stage it's copies are issued: their latency was exposed once per stage)
-          int ra[4], rb[4];
+  if (warp < 4) {
+    if (warp == 0 && GATHER) {
+      // ===================================================================== gather producer (whole warp) + weight TMA
+      const uint32_t txb = 2 * B_BYTES;
+      int ig = 0;
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
+        int nt, mt, tap, count, kb, ke;
+        decode(pt, nt, mt, tap, count, kb, ke);
+        const int n0 = nt * BN;
+        const int* pin = GM == 1 ? p.pairs_in + (long long)tap * p.pair_cap : nullptr;
+        int rows[4];
+        int nxa[4] = {-1, -1, -1, -1}, nxb[4] = {-1, -1, -1, -1};   // neighbour indices of the next stage / tap (GM == 2)
+        if (GM == 1) {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            if (it == kb) {
-              const int m = mt * BM + lane + 32 * i;
-              const int* nb = p.nbr + (long long)m * p.kvol + 2 * it;
-              ra[i] = m < count ? __ldg(nb) : -1;
-              rb[i] = (m < count && 2 * it + 1 < p.kvol) ? __ldg(nb + 1) : -1;
-            } else {
-              ra[i] = nxa[i]; rb[i] = nxb[i];
-            }
+            const int m = mt * BM + lane + 32 * i;
+            rows[i] = m < count ? __ldg(pin + m) : -1;
           }
-          if (it + 1 < ke) {
+        }
+        for (int it = kb; it < ke; ++it, ++ig) {
+          const int s = ig % STAGES;
+          if (GM == 2 && p.tps == 2) {
+            // ---- two taps per K slab (Cin = 32): chunks 0..3 of a row come from the neighbour under tap 2 it, chunks 4..7 from tap 2 it + 1
+            // (the neighbour indices of stage it + 1 are fetched while stage it's copies are issued)
+            int ra[4], rb[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              if (it == kb) {
+                const int m = mt * BM + lane + 32 * i;
+                const int* nb = p.nbr + (long long)m * p.kvol + 2 * it;
+                ra[i] = m < count ? __ldg(nb) : -1;
+                rb[i] = (m < count && 2 * it + 1 < p.kvol) ? __ldg(nb + 1) : -1;
+              } else {
+                ra[i] = nxa[i]; rb[i] = nxb[i];
+              }
+            }
+            if (it + 1 < ke) {
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int m = mt * BM + lane + 32 * i;
+                const int* nb = p.nbr + (long long)m * p.kvol + 2 * (it + 1);
+                nxa[i] = m < count ? __ldg(nb) : -1;
+                nxb[i] = (m < count && 2 * (it + 1) + 1 < p.kvol) ? __ldg(nb + 1) : -1;
+              }
+            }
+            mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
+            uint8_t* st = smem + s * STAGE_BYTES;
+            if (lane == 0) {
+              mbar_expect_tx(&full[s], txb);
+              load_weights(st, &full[s], it * KE, 0, n0);              // weights viewed as [Cout][kvol * 32]: K runs across the taps
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int r = lane + 32 * i;
+              const uint32_t dst = smem_u32(st) + r * 128;
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const int row = j < 4 ? ra[i] : rb[i];
+                const bool ok = row >= 0;
+                const __half* src = p.gx + (long long)max(row, 0) * p.gx_ld + (j & 3) * 8;
+                const uint32_t o = (uint32_t)((j ^ (r & 7)) << 4);
+                cp_async16(dst + o, ok ? (const void*)src : (const void*)p.gx, ok ? 16 : 0);
+                cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane) : (const void*)p.gx, ok ? 16 : 0);
+              }
+            }
+            cp_async_arrive_noinc(&full[s]);
+            continue;
+          }
+          const int ktap = GM == 2 ? it / p.n_slabs : tap;            // output-stationary: the K walk visits every tap
+          const int slab = GM == 2 ? it - ktap * p.n_slabs : it;
+          if (GM == 2 && (slab == 0 || it == kb)) {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int m = mt * BM + lane + 32 * i;
-              const int* nb = p.nbr + (long long)m * p.kvol + 2 * (it + 1);
-              nxa[i] = m < count ? __ldg(nb) : -1;
-              nxb[i] = (m < count && 2 * (it + 1) + 1 < p.kvol) ? __ldg(nb + 1) : -1;
+              if (it == kb) rows[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap) : -1;       // -1: no input site under this tap
+              else rows[i] = nxa[i];                                                                       // fetched one tap ahead
+            }
+            if (ktap + 1 < taps) {                              // next tap's neighbours: in flight while this tap's copies are issued
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const int m = mt * BM + lane + 32 * i;
+                nxa[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap + 1) : -1;
+              }
             }
           }
           mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
           uint8_t* st = smem + s * STAGE_BYTES;
           if (lane == 0) {
             mbar_expect_tx(&full[s], txb);
-            load_weights(st, &full[s], it * KE, 0, n0);              // weights viewed as [Cout][kvol * 32]: K runs across the taps
+            load_weights(st, &full[s], slab * KE, ktap, n0);
           }
+          const int c0 = slab * KE;
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const int r = lane + 32 * i;
+            const __half* src = p.gx + (long long)max(rows[i], 0) * p.gx_ld + c0;
             const uint32_t dst = smem_u32(st) + r * 128;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int row = j < 4 ? ra[i] : rb[i];
-              const bool ok = row >= 0;
-              const __half* src = p.gx + (long long)max(row, 0) * p.gx_ld + (j & 3) * 8;
+            for (int j = 0; j < 8; ++j) {                       // 16-byte chunk j (8 halves) of row r lives at chunk j ^ (r & 7)
+              const bool ok = rows[i] >= 0 && c0 + j * 8 < d.Cin;
               const uint32_t o = (uint32_t)((j ^ (r & 7)) << 4);
-              cp_async16(dst + o, ok ? (const void*)src : (const void*)p.gx, ok ? 16 : 0);
-              cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane) : (const void*)p.gx, ok ? 16 : 0);
+              cp_async16(dst + o, ok ? (const void*)(src + j * 8) : (const void*)p.gx, ok ? 16 : 0);
+              cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane + j * 8) : (const void*)p.gx, ok ? 16 : 0);
             }
           }
           cp_async_arrive_noinc(&full[s]);
-          continue;
         }
-        const int ktap = GM == 2 ? it / p.n_slabs : tap;            // output-stationary: the K walk visits every tap
-        const int slab = GM == 2 ? it - ktap * p.n_slabs : it;
-        if (GM == 2 && (slab == 0 || it == kb)) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int m = mt * BM + lane + 32 * i;
-            if (it == kb) rows[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap) : -1;       // -1: no input site under this tap
-            else rows[i] = nxa[i];                                                                       // fetched one tap ahead
-          }
-          if (ktap + 1 < taps) {                              // next tap's neighbours: in flight while this tap's copies are issued
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int m = mt * BM + lane + 32 * i;
-              nxa[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap + 1) : -1;
-            }
-          }
-        }
-        mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
-        uint8_t* st = smem + s * STAGE_BYTES;
-        if (lane == 0) {
-          mbar_expect_tx(&full[s], txb);
-          load_weights(st, &full[s], slab * KE, ktap, n0);
-        }
-        const int c0 = slab * KE;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int r = lane + 32 * i;
-          const __half* src = p.gx + (long long)max(rows[i], 0) * p.gx_ld + c0;
-          const uint32_t dst = smem_u32(st) + r * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {                       // 16-byte chunk j (8 halves) of row r lives at chunk j ^ (r & 7)
-            const bool ok = rows[i] >= 0 && c0 + j * 8 < d.Cin;
-            const uint32_t o = (uint32_t)((j ^ (r & 7)) << 4);
-            cp_async16(dst + o, ok ? (const void*)(src + j * 8) : (const void*)p.gx, ok ? 16 : 0);
-            cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane + j * 8) : (const void*)p.gx, ok ? 16 : 0);
-          }
-        }
-        cp_async_arrive_noinc(&full[s]);
       }
-    }
-  } else if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
+    } else if (warp == 0 && lane == 0) {
+      // ===================================================================== TMA producer
       const uint32_t a_box = (uint32_t)(p.flat ? BM : p.TH * p.TW) * KE * 2;   // bytes one activation box (one plane) delivers
-      const uint32_t tx = ((p.dbg & 2) ? 0u : 2 * a_box) + (CG == 2 ? (uint32_t)(B_BYTES + B_BYTES / 2) : 2 * B_BYTES);
+      const uint32_t tx = 2 * a_box + 2 * B_BYTES;
       int ig = 0;
-      for (int pt = pair0; pt < total_pairs; pt += pair_step) {
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
         int nt, mt, tap0, count, kb, ke;
         decode(pt, nt, mt, tap0, count, kb, ke);
         const int n0 = nt * BN;
@@ -418,358 +314,175 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           uint8_t* st = smem + s * STAGE_BYTES;
           const int tap = it / p.n_slabs, slab = it - tap * p.n_slabs;
           const int kh = tap / d.KW, kw = tap - kh * d.KW;
-          if constexpr (CG == 2) {
-            // every load of BOTH CTAs completes on the leader's barrier: the leader announces the pair's bytes, the peer only loads
-            // (its complete_tx may land before the announcement: the barrier's pending arrival keeps the phase open)
-            if (rank == 0) mbar_expect_tx(&full[s], 2 * tx);
-            if (!(p.dbg & 2)) {
-              if (p.flat) {
-                tma2_load_3d(st, &map_a, &full[s], slab * KE, cw0, 0);
-                tma2_load_3d(st + A_BYTES, &map_a, &full[s], slab * KE, cw0, 1);
-              } else {
-                const int cw = cw0 + kw * d.dil, ch = ch0 + kh * d.dil;
-                tma2_load_5d(st, &map_a, &full[s], slab * KE, cw, ch, cn, 0);
-                tma2_load_5d(st + A_BYTES, &map_a, &full[s], slab * KE, cw, ch, cn, 1);
-              }
-            }
-            uint8_t* bb = st + 2 * A_BYTES;                           // 128-row block: plane `rank` (hi in the leader, lo' in the peer)
-            tma2_load_4d(bb, &map_b, &full[s], slab * KE, tap, n0, (int)rank);
-            tma2_load_4d(bb + B_BYTES / 2, &map_b, &full[s], slab * KE, tap, n0 + BN / 2, (int)rank);
-            tma2_load_4d(bb + B_BYTES, &map_b, &full[s], slab * KE, tap, n0 + (int)rank * (BN / 2), 0);   // this CTA's half of B_hi
-            continue;
-          }
-          if ((p.dbg & 8) && ig >= STAGES) {                   // diagnosis: no loads after the ring's first fill (stale operands)
-            asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full[s])) : "memory");
-            continue;
-          }
           mbar_expect_tx(&full[s], tx);
-          if (!(p.dbg & 2)) {
-            if (p.flat) {
-              tma_load_3d(st, &map_a, &full[s], slab * KE, cw0, 0);
-              tma_load_3d(st + A_BYTES, &map_a, &full[s], slab * KE, cw0, 1);
-            } else {
-              const int cw = cw0 + kw * d.dil, ch = ch0 + kh * d.dil;
-              tma_load_5d(st, &map_a, &full[s], slab * KE, cw, ch, cn, 0);
-              tma_load_5d(st + A_BYTES, &map_a, &full[s], slab * KE, cw, ch, cn, 1);
-            }
+          if (p.flat) {
+            tma_load_3d(st, &map_a, &full[s], slab * KE, cw0, 0);
+            tma_load_3d(st + A_BYTES, &map_a, &full[s], slab * KE, cw0, 1);
+          } else {
+            const int cw = cw0 + kw * d.dil, ch = ch0 + kh * d.dil;
+            tma_load_5d(st, &map_a, &full[s], slab * KE, cw, ch, cn, 0);
+            tma_load_5d(st + A_BYTES, &map_a, &full[s], slab * KE, cw, ch, cn, 1);
           }
           load_weights(st, &full[s], slab * KE, tap, n0);
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (one thread; cta_group::2: of the pair's leader only)
-    if (lane == 0 && (CG == 1 || rank == 0)) {
-      constexpr uint32_t idesc = make_idesc_f16(CG * BM, BN);
-      constexpr uint32_t idesc2 = make_idesc_f16(CG * BM, 2 * BN);
-      int ig = 0, cg = 0, tg = 0;
-      // corr_once: the correction products (hi x lo' + lo' x hi, weighted 2^-11 in the result) tolerate the truncating accumulation
-      // of the tensor core over the WHOLE K walk — their rounding error is 2^-11 times smaller than the main product's — so only
-      // the main accumulator is folded into fp32 registers every `chunk` stages; the correction accumulator of work item t lives in
-      // buffer t & 1 until the item's last chunk.  Halves the TMEM read traffic of the drains (TMEM reads are 64 B / clk / SM:
-      // 128 KB per K = 128 chunk was 2048 clk against 1536 clk of MMA) at the price of a third N = BN instruction per K step.
-      for (int pt = pair0; pt < total_pairs; pt += pair_step, ++tg) {
-        int nt, mt, tap0, count, kb, ke;
-        decode(pt, nt, mt, tap0, count, kb, ke);
-        int it = kb;
-        const int nch = (ke - kb + p.chunk - 1) / p.chunk;
-        const uint32_t t_corr1 = tmem_base + (uint32_t)((tg & 1) * ACC_COLS + BN);
-        if constexpr (CO) {
-          mbar_wait(&corr_empty[tg & 1], ((tg >> 1) & 1) ^ 1);
-          tcgen05_fence_after();
-        }
-        bool first_of_item = true;
-        for (int c = 0; c < nch; ++c, ++cg) {
-          const int b = cg & 1;
-          mbar_wait(&acc_empty[b], ((cg >> 1) & 1) ^ 1);
-          tcgen05_fence_after();
-          const uint32_t t_main = tmem_base + (uint32_t)(b * ACC_COLS), t_corr = t_main + BN;
-          const int it_end = min(it + p.chunk, ke);
-          bool first = true;
-          for (; it < it_end; ++it, ++ig) {
-            const int s = ig % STAGES;
-            mbar_wait(&full[s], (ig / STAGES) & 1);
-            tcgen05_fence_after();
-            const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES), a_lo = a_hi + A_BYTES;
-            const uint32_t b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-#pragma unroll
-            for (int kk = 0; kk < KE / 16; ++kk) {           // UMMA K = 16 halves = 32 bytes inside the 128-byte swizzle row
-              if (p.dbg & 4) break;
-              const uint32_t off = kk * 32;
-              const uint32_t acc = (first && kk == 0) ? 0u : 1u;
-              if constexpr (CO) {
-                umma_f16(t_main, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), idesc, acc);                           // hi*hi
-                umma_f16(t_corr1, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), idesc, (first_of_item && kk == 0) ? 0u : 1u);   // hi*lo'
-                umma_f16(t_corr1, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), idesc, 1);                            // lo'*hi
-              } else if constexpr (CG == 2) {
-                // M = 256 over the pair; B rows split between the CTAs: [B_hi (leader) ; B_lo' (peer)] and the two halves of B_hi
-                umma_f16_2cta(t_main, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), idesc2, acc);            // hi*hi | hi*lo'
-                umma_f16_2cta(t_corr, make_smem_desc(a_lo + off), make_smem_desc(b_hi + B_BYTES + off), idesc, 1);     // lo'*hi
-              } else {
-                umma_f16(t_main, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), idesc2, acc);   // hi*hi | hi*lo'
-                umma_f16(t_corr, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), idesc, 1);      // lo'*hi
-              }
-            }
-            first = false;
-            first_of_item = false;
-            if constexpr (CG == 2) tcgen05_commit_2cta(&empty[s]);
-            else if (PAIR) tcgen05_commit_mc(&empty[s], 3);
-            else tcgen05_commit(&empty[s]);
-          }
-          if constexpr (CG == 2) tcgen05_commit_2cta(&acc_full[b]); else tcgen05_commit(&acc_full[b]);
-        }
-      }
-    }
   } else {
-    // ===================================================================== epilogue (warps 2..9)
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
+    // ===================================================================== MMA + epilogue (warpgroups 1, 2)
+    const int cw = warp - 4;                                // MMA warp 0..7
+    const int wg = cw >> 2;                                 // warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int row0 = wg * 64 + (cw & 3) * 16;               // this warp's 16 accumulator rows
     const long long yns = d.y_nstride ? d.y_nstride : (long long)d.yH * d.yW * d.y_ld;
     const int HWo = d.OH * d.OW;
-    float* tile = tile_all + (warp - 2) * RPP * PITCH;
+    float* tile = tile_all + cw * 16 * PITCH;               // warp-private transposition buffer [16 rows][PITCH]
+    const int sub = lane >> 2, cl = (lane & 3) * 4;         // store phase: 4 lanes per row, 8 rows per warp instruction
     bool sat = false;
-    int cg = 0, tg = 0;
-    for (int pt = pair0; pt < total_pairs; pt += pair_step, ++tg) {
+    int ig = 0;
+    for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
       int nt, mt, tap, count, kb, ke;
       decode(pt, nt, mt, tap, count, kb, ke);
       const int nch = (ke - kb + p.chunk - 1) / p.chunk;
       const bool real_tile = GATHER ? mt * BM < count : mt < p.m_tiles;
-      const int n0 = nt * BN + half * HN;
-      if (GM == 2) {
+      const int n0 = nt * BN;
+      // ---- output / residual addresses of the two rows this lane stores (rows row0 + sub, row0 + 8 + sub)
+      int fl[2];
+      long long yo[2], o1[2], o2[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = row0 + i * 8 + sub;
         const int m = mt * BM + r;
-        const bool valid = m < count;
-        const long long r1 = (long long)m * d.res_ld + d.res_coff;
-        if (half == 0) {
-          row_y[r] = (long long)m * d.y_ld + d.y_coff;
-          row_r1[r] = r1;
-          row_r2[r] = 0;
-          row_flag[r] = valid ? 1 : 0;
-        }
-      } else if (GM == 1) {
-        const int m = mt * BM + r;
-        const bool valid = m < count;
-        if (half == 0) {
+        o2[i] = 0;
+        if (GM == 2) {
+          fl[i] = m < count ? 1 : 0;
+          yo[i] = (long long)m * d.y_ld + d.y_coff;
+          o1[i] = (long long)m * d.res_ld + d.res_coff;
+        } else if (GM == 1) {
+          const bool valid = m < count;
           const int orow = valid ? __ldg(p.pairs_out + (long long)tap * p.pair_cap + m) : 0;
-          row_y[r] = (long long)orow * d.y_ld + d.y_coff;
-          row_r1[r] = 0;
-          row_r2[r] = 0;
-          row_flag[r] = valid ? 1 : 0;
-        }
-      } else {
-        bool valid;
-        int nimg, oh, ow;
-        long long rrow;
-        if (p.flat) {
-          const int pix = mt * BM + r;                       // (the host checked N * OH * OW < 2^31: 32-bit index math)
-          valid = real_tile && pix < p.total_pix;
-          nimg = pix / HWo;
-          const int rem = pix - nimg * HWo;
-          oh = rem / d.OW; ow = rem - oh * d.OW;
-          rrow = pix;
+          fl[i] = valid ? 1 : 0;
+          yo[i] = (long long)orow * d.y_ld + d.y_coff;
+          o1[i] = 0;
         } else {
-          const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h;
-          nimg = mt / (p.tiles_w * p.tiles_h);
-          const int rh = r / p.TW, rw = r - rh * p.TW;
-          oh = th * p.TH + rh; ow = tw * p.TW + rw;
-          valid = real_tile && (r < p.TH * p.TW) && oh < d.OH && ow < d.OW;
-          rrow = ((long long)nimg * d.OH + oh) * d.OW + ow;
-        }
-        const long long r1 = (d.res_mode == TT_RES_UP2_NEAREST
-                                  ? ((long long)nimg * d.res_H + (oh * d.res_H) / d.OH) * d.res_W + (ow * d.res_W) / d.OW
-                                  : rrow) * d.res_ld + d.res_coff;
-        const long long r2 = rrow * d.res2_ld + d.res2_coff;
-        if (half == 0) {
-          row_y[r] = nimg * yns + ((long long)(oh * d.oy_mul + d.oy_add) * d.yW + ow * d.ox_mul + d.ox_add) * d.y_ld + d.y_coff;
-          row_r1[r] = r1;
-          row_r2[r] = r2;
-          row_flag[r] = (valid ? 1 : 0) | (nimg << 1);
-        }
-        if (valid && n0 < d.Cout) {
-          if (p.res) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res + r1 + n0 + j));
-          } else if (p.res_s) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 64) {
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res_s + r1 + n0 + j));
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res_s + p.res_plane + r1 + n0 + j));
-            }
-          }
-          if (p.res2) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res2 + r2 + n0 + j));
-          } else if (p.res2_s) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 64) {
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res2_s + r2 + n0 + j));
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res2_s + p.res2_plane + r2 + n0 + j));
-            }
-          }
-        }
-      }
-      float sum[HN];
-#pragma unroll
-      for (int j = 0; j < HN; ++j) sum[j] = 0.f;
-      for (int c = 0; c < nch; ++c, ++cg) {
-        const int b = cg & 1;
-        mbar_wait(&acc_full[b], (cg >> 1) & 1);
-        tcgen05_fence_after();
-        const uint32_t t_main = tmem_base + lane_addr + (uint32_t)(b * ACC_COLS + half * HN);
-        if constexpr (CO) {                                    // main accumulator only: the correction stays in TMEM until the last chunk
-          if constexpr (EW == 16) {
-#pragma unroll
-            for (int c0 = 0; c0 < HN; c0 += 16) {
-              uint32_t v[16];
-              tmem_ld16(t_main + c0, v);
-#pragma unroll
-              for (int j = 0; j < 16; ++j) sum[c0 + j] += __uint_as_float(v[j]);
-            }
+          bool valid;
+          int nimg, oh, ow;
+          long long rrow;
+          if (p.flat) {
+            const int pix = m;                                 // (the host checked N * OH * OW < 2^31: 32-bit index math)
+            valid = real_tile && pix < p.total_pix;
+            nimg = pix / HWo;
+            const int rem = pix - nimg * HWo;
+            oh = rem / d.OW; ow = rem - oh * d.OW;
+            rrow = pix;
           } else {
-#pragma unroll
-            for (int c0 = 0; c0 < HN; c0 += 32) {
-              uint32_t v[32];
-              tmem_ld32(t_main + c0, v);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) sum[c0 + j] += __uint_as_float(v[j]);                          // fp32 RN
-            }
+            const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h;
+            nimg = mt / (p.tiles_w * p.tiles_h);
+            const int rh = r / p.TW, rw = r - rh * p.TW;
+            oh = th * p.TH + rh; ow = tw * p.TW + rw;
+            valid = real_tile && (r < p.TH * p.TW) && oh < d.OH && ow < d.OW;
+            rrow = ((long long)nimg * d.OH + oh) * d.OW + ow;
           }
-        } else if constexpr (EW == 16) {                       // register budget of the 576-thread variant: 16 columns at a time
-#pragma unroll
-          for (int c0 = 0; c0 < HN; c0 += 16) {
-            uint32_t v[16], u[16];
-            tmem_ld16(t_main + c0, v);
-            tmem_ld16(t_main + BN + c0, u);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) sum[c0 + j] += fmaf(__uint_as_float(u[j]), LO_INV, __uint_as_float(v[j]));
-          }
-        } else if (!(p.dbg & 16)) {                            // (knob 16: diagnosis — barriers only, no TMEM reads)
-#pragma unroll
-          for (int c0 = 0; c0 < HN; c0 += 32) {
-            uint32_t v[32], u[32];
-            tmem_ld32(t_main + c0, v);
-            tmem_ld32(t_main + BN + c0, u);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) sum[c0 + j] += fmaf(__uint_as_float(u[j]), LO_INV, __uint_as_float(v[j]));   // fp32 RN
-          }
+          o1[i] = (d.res_mode == TT_RES_UP2_NEAREST
+                       ? ((long long)nimg * d.res_H + (oh * d.res_H) / d.OH) * d.res_W + (ow * d.res_W) / d.OW
+                       : rrow) * d.res_ld + d.res_coff;
+          o2[i] = rrow * d.res2_ld + d.res2_coff;
+          yo[i] = nimg * yns + ((long long)(oh * d.oy_mul + d.oy_add) * d.yW + ow * d.ox_mul + d.ox_add) * d.y_ld + d.y_coff;
+          fl[i] = (valid ? 1 : 0) | (nimg << 1);
         }
-        tcgen05_fence_before();
+      }
+      // ---- K walk: chunks of `chunk` stages accumulated by the tensor core, folded into fp32 sums with RN FMAs
+      float sum[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
+      auto release = [&](int s) {                            // this warp's wgmmas no longer read stage s
         __syncwarp();
-        if (lane == 0) {
-          if constexpr (CG == 2) mbar_arrive_leader(&acc_empty[b]);        // the pair's MMA issuer waits for BOTH CTAs' drains
-          else asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[b])) : "memory");
-        }
-      }
-      if constexpr (CO) {
-        // every MMA of this work item is complete (the last chunk's commit covered them): fold the correction accumulator in, once
-        const uint32_t t_corr = tmem_base + lane_addr + (uint32_t)((tg & 1) * ACC_COLS + BN + half * HN);
-        if constexpr (EW == 16) {
+        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
+      };
+      int it = kb;
+      for (int c = 0; c < nch; ++c) {
+        float acc[BN / 2], cor[BN / 2];                      // main and correction accumulators
+        const int it_end = min(it + p.chunk, ke);
+        int held = -1;                                       // the stage whose wgmmas may still be in flight
+        for (bool first = true; it < it_end; ++it, ++ig, first = false) {
+          const int s = ig % STAGES;
+          mbar_wait(&full[s], (ig / STAGES) & 1);
+          if (GATHER) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async rows -> visible to wgmma
+          const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES) + wg * (A_BYTES / 2), a_lo = a_hi + A_BYTES;
+          const uint32_t b_hi = smem_u32(smem + s * STAGE_BYTES) + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+          wgmma_fence();
 #pragma unroll
-          for (int c0 = 0; c0 < HN; c0 += 16) {
-            uint32_t u[16];
-            tmem_ld16(t_corr + c0, u);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) sum[c0 + j] = fmaf(__uint_as_float(u[j]), LO_INV, sum[c0 + j]);
+          for (int kk = 0; kk < KE / 16; ++kk) {             // K = 16 halves = 32 bytes inside the 128-byte swizzle row
+            const uint32_t off = kk * 32, z = (first && kk == 0) ? 0u : 1u;
+            wgmma_f16<BN>(acc, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), z);    // hi*hi
+            wgmma_f16<BN>(cor, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), z);    // hi*lo'
+            wgmma_f16<BN>(cor, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), 1u);   // lo'*hi
           }
-        } else {
-#pragma unroll
-          for (int c0 = 0; c0 < HN; c0 += 32) {
-            uint32_t u[32];
-            tmem_ld32(t_corr + c0, u);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) sum[c0 + j] = fmaf(__uint_as_float(u[j]), LO_INV, sum[c0 + j]);
+          wgmma_commit();
+          if (held >= 0) {                                   // one stage stays in flight: the previous one is complete now
+            wgmma_wait<1>();
+            release(held);
           }
+          held = s;
         }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&corr_empty[tg & 1])) : "memory");
-      }
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
-      const int sub = lane >> 2, cl = (lane & 3) * 4;
-      // the 4 rows this lane stores (row groups of 8) are the same for every column slab: their table entries are read ONCE
-      // per tile into registers (the profile showed the per-slab table reloads and the residual round trips as the epilogue's
-      // long-scoreboard stalls on the short-K layers, where the epilogue sets the pace: profiles/r2_summary.md)
-      int fl[4];
-      long long yo[4], o1[4], o2[4];
+        wgmma_wait<0>();
+        release(held);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int rr = q * 32 + i * 8 + sub;
-        fl[i] = row_flag[rr];
-        yo[i] = row_y[rr];
-        o1[i] = row_r1[rr];
-        o2[i] = row_r2[rr];
+        for (int j = 0; j < BN / 2; ++j) sum[j] += fmaf(cor[j], LO_INV, acc[j]);
       }
+      // ---- coalesced store in 16-column slabs: registers -> warp-private smem (transpose) -> 64-byte row segments
 #pragma unroll
-      for (int sl = 0; sl < HN / SLAB; ++sl) {
+      for (int sl = 0; sl < BN / SLAB; ++sl) {
         const int col = n0 + sl * SLAB + cl;
-        const bool live = col < d.Cout && !(p.dbg & 1);
+        const bool live = col < d.Cout;
         // residual / bias loads of this slab are issued BEFORE the shared-memory transposition so that the two latencies overlap
-        // (a deeper software pipeline — loads one slab ahead — pushed the staging arrays into local memory and cost 25 %: measured)
-        float4 ra[4], rb[4];
+        float4 ra[2], rb[2];
         float4 bv0 = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < 2; ++i) {
           ra[i] = make_float4(0.f, 0.f, 0.f, 0.f);
           rb[i] = ra[i];
           if (live && (fl[i] & 1)) {
             if (p.res) ra[i] = *reinterpret_cast<const float4*>(p.res + o1[i] + col);
             else if (p.res_s) ra[i] = load_split4(p.res_s + o1[i] + col, p.res_plane);
-            if constexpr (EW != 16) {                           // (the 16-warp variant is not launched for layers with a second residual)
-              if (p.res2) rb[i] = *reinterpret_cast<const float4*>(p.res2 + o2[i] + col);
-              else if (p.res2_s) rb[i] = load_split4(p.res2_s + o2[i] + col, p.res2_plane);
-            }
+            if (p.res2) rb[i] = *reinterpret_cast<const float4*>(p.res2 + o2[i] + col);
+            else if (p.res2_s) rb[i] = load_split4(p.res2_s + o2[i] + col, p.res2_plane);
           }
         }
         if (live && p.bias && !d.bias_n_mod) bv0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));   // one bias vector: once per slab
+        __syncwarp();
 #pragma unroll
-        for (int ph = 0; ph < 32 / RPP; ++ph) {
-          __syncwarp();
-          if (lane / RPP == ph) {                                // (RPP == 32: every lane) this lane's row goes through the buffer now
+        for (int jj = 0; jj < 2; ++jj) {                     // fragment column group j = 2 sl + jj: columns 8 jj + 2 (lane % 4) + {0, 1}
+          const int j = 2 * sl + jj, cc = 8 * jj + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(&tile[sub * PITCH + cc]) = make_float2(sum[4 * j], sum[4 * j + 1]);
+          *reinterpret_cast<float2*>(&tile[(sub + 8) * PITCH + cc]) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
+        }
+        __syncwarp();
+        if (live) {
 #pragma unroll
-            for (int j = 0; j < SLAB; j += 4)
-              *reinterpret_cast<float4*>(&tile[(lane % RPP) * PITCH + j]) =
-                  make_float4(sum[sl * SLAB + j], sum[sl * SLAB + j + 1], sum[sl * SLAB + j + 2], sum[sl * SLAB + j + 3]);
-          }
-          __syncwarp();
-          if (live) {
-#pragma unroll
-            for (int ii = 0; ii < RPP / 8; ++ii) {
-              const int i = ph * (RPP / 8) + ii;
-              if (!(fl[i] & 1)) continue;
-              const float4 acc4 = *reinterpret_cast<const float4*>(&tile[(ii * 8 + sub) * PITCH + cl]);
-              float4 bv = bv0;
-              if (p.bias && d.bias_n_mod) bv = __ldg(reinterpret_cast<const float4*>(p.bias + (long long)((fl[i] >> 1) % d.bias_n_mod) * d.Cout + col));
-              float4 o = make_float4(acc4.x + bv.x + ra[i].x + rb[i].x, acc4.y + bv.y + ra[i].y + rb[i].y,
-                                     acc4.z + bv.z + ra[i].z + rb[i].z, acc4.w + bv.w + ra[i].w + rb[i].w);
-              const long long eo = yo[i] + col;
-              if (GM == 1 || p.splits > 1) {                     // taps / K splits race on an output row: red.add (fp32 only)
-                tt_red_add_v4(p.y + eo, o.x, o.y, o.z, o.w);
-              } else {
-                o = make_float4(tt_act(o.x, d.act), tt_act(o.y, d.act), tt_act(o.z, d.act), tt_act(o.w, d.act));
-                if (p.y) *reinterpret_cast<float4*>(p.y + eo) = o;
-                if (p.ys) {
-                  uint2 hi, lo;
-                  split4(o, hi, lo, sat);
-                  *reinterpret_cast<uint2*>(p.ys + eo) = hi;
-                  *reinterpret_cast<uint2*>(p.ys + p.ys_plane + eo) = lo;
-                }
+          for (int i = 0; i < 2; ++i) {
+            if (!(fl[i] & 1)) continue;
+            const float4 acc4 = *reinterpret_cast<const float4*>(&tile[(i * 8 + sub) * PITCH + cl]);
+            float4 bv = bv0;
+            if (p.bias && d.bias_n_mod) bv = __ldg(reinterpret_cast<const float4*>(p.bias + (long long)((fl[i] >> 1) % d.bias_n_mod) * d.Cout + col));
+            float4 o = make_float4(acc4.x + bv.x + ra[i].x + rb[i].x, acc4.y + bv.y + ra[i].y + rb[i].y,
+                                   acc4.z + bv.z + ra[i].z + rb[i].z, acc4.w + bv.w + ra[i].w + rb[i].w);
+            const long long eo = yo[i] + col;
+            if (GM == 1 || p.splits > 1) {                     // taps / K splits race on an output row: red.add (fp32 only)
+              tt_red_add_v4(p.y + eo, o.x, o.y, o.z, o.w);
+            } else {
+              o = make_float4(tt_act(o.x, d.act), tt_act(o.y, d.act), tt_act(o.z, d.act), tt_act(o.w, d.act));
+              if (p.y) *reinterpret_cast<float4*>(p.y + eo) = o;
+              if (p.ys) {
+                uint2 hi, lo;
+                split4(o, hi, lo, sat);
+                *reinterpret_cast<uint2*>(p.ys + eo) = hi;
+                *reinterpret_cast<uint2*>(p.ys + p.ys_plane + eo) = lo;
               }
             }
           }
         }
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * EW) : "memory");
     }
     if (sat) atomicAdd(&g_f16s_saturated, 1u);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if constexpr (CG == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
   }
 }
 
@@ -1023,49 +736,24 @@ __global__ void f16s_sparse_init_kernel(float* __restrict__ y, int y_ld, const f
   }
 }
 
-int num_sms_cached() {
-  static int n = 0;
-  if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); }
-  return n;
-}
-constexpr int EPI_BYTES = 8 * 32 * 20 * 4 + BM * (3 * 8 + 4) + 512;
+// shared memory beyond the stage ring: 8 warp-private transposition slabs, barriers and the tap prefix
+constexpr int EPI_BYTES = 8 * 16 * 20 * 4 + 512;
+// N tile: each MMA thread holds BN fp32 accumulators (BN / 2 main + BN / 2 corr) plus BN / 2 fp32 sums; at 384 threads
+// per CTA the compiler's budget is 168 registers per thread, which BN = 128 (192 live accumulators) overflows
+constexpr int BN = 64, STAGES = 4;
 
-template <int BN, int STAGES, int GATHER, bool PAIR, int EW, bool CO, int CG = 1>
-cudaError_t launch_f16s_co(cudaLaunchConfig_t& cfg, const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a) {
-  constexpr int smem = STAGES * (2 * BM * KE * 2 + (CG == 2 ? 3 : 4) * BN * KE) + 1024 + EPI_BYTES;
+// persistent grid: one CTA per SM walks the (M unit, N tile, K split) work items; debug bits 8..15: SMs left to a concurrent branch
+template <int GM>
+cudaError_t launch_f16s(const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a, long long m_units, cudaStream_t st) {
+  constexpr int smem = STAGES * (2 * BM * KE * 2 + 2 * BN * KE * 2) + 1024 + EPI_BYTES;
+  static_assert(smem <= 227 * 1024, "shared memory per block");
   static bool set = false;
-  if (!set) { cudaFuncSetAttribute(conv_f16s_kernel<BN, STAGES, GATHER, PAIR, EW, CO, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set = true; }
-  cfg.dynamicSmemBytes = smem;
-  cfg.blockDim = dim3(64 + 32 * EW);
-  return cudaLaunchKernelEx(&cfg, conv_f16s_kernel<BN, STAGES, GATHER, PAIR, EW, CO, CG>, ma, mb, a);
-}
-template <int BN, int STAGES, int GATHER, bool PAIR, int EW = 8>
-cudaError_t launch_f16s_v(cudaLaunchConfig_t& cfg, const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a) {
-  return a.corr_once ? launch_f16s_co<BN, STAGES, GATHER, PAIR, EW, true>(cfg, ma, mb, a) : launch_f16s_co<BN, STAGES, GATHER, PAIR, EW, false>(cfg, ma, mb, a);
-}
-// work items / grid for `tiles` M tiles; debug bit 0x100000 selects the unpaired variant
-template <int BN, int STAGES, int GATHER>
-cudaError_t launch_f16s(cudaLaunchConfig_t& cfg, const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a, long long m_units) {
-  const bool pair = !(g_tt_debug & 0x100000);
-  const int cl = pair ? 2 : 1;
-  const int num_sms = num_sms_cached() - ((g_tt_debug >> 8) & 0xFF);
-  const long long items = ((m_units + cl - 1) / cl) * a.n_tiles * a.splits;
-  const long long max_items = num_sms / cl;
-  cfg.gridDim = dim3((unsigned)(cl * (items < max_items ? items : max_items)));
-  cfg.attrs[0].val.clusterDim.x = cl;
-  // 16 epilogue warps for the 1x1 layers (dense BN = 128 tiles): with one to four K stages per tile the epilogue sets the pace, and
-  // twice the warps hide its store / residual latencies (measured +17..22 % on 64->256 / 256->256 @112x224, +7 % on 2048->512); the
-  // 3x3 trunk layers keep 8 (256->256 @112x224: -6 % with 16).  Debug bit 0x400000 turns the variant off.
-  if constexpr (GATHER == 0) {
-    if (pair && a.d.KH * a.d.KW == 1 && !(g_tt_debug & 0x400000) && !a.res2 && !a.res2_s) return launch_f16s_v<BN, STAGES, GATHER, true, 16>(cfg, ma, mb, a);
-  }
-  // cta_group::2 (one MMA of the pair's leader over M = 256, each SM reading only half of the weight rows).  Measured (profiles/r2_summary.md):
-  // parity green, no gain on the long-K layers (341 -> 336 us; 8 x images: slower) — their pace is set by the barrier ring and the epilogue's
-  // store phase, not by the operand reads.  Kept behind debug bit 0x2000000 as the starting point of a deeper-pipelined pair kernel.
-  if constexpr (GATHER == 0 && BN == 128) {
-    if (pair && (g_tt_debug & 0x2000000) && !a.corr_once) return launch_f16s_co<BN, STAGES, GATHER, true, 8, false, 2>(cfg, ma, mb, a);
-  }
-  return pair ? launch_f16s_v<BN, STAGES, GATHER, true>(cfg, ma, mb, a) : launch_f16s_v<BN, STAGES, GATHER, false>(cfg, ma, mb, a);
+  if (!set) { cudaFuncSetAttribute(conv_f16s_kernel<BN, STAGES, GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set = true; }
+  const long long num_sms = tt_num_sms() - ((g_tt_debug >> 8) & 0xFF);
+  const long long items = m_units * a.n_tiles * a.splits;
+  const long long grid = items < num_sms ? items : num_sms;
+  conv_f16s_kernel<BN, STAGES, GM><<<(unsigned)(grid > 1 ? grid : 1), NTHREADS, smem, st>>>(ma, mb, a);
+  return cudaGetLastError();
 }
 
 bool encode_weights(CUtensorMap* mb, const void* w_split, int Cin, int taps, int Cout, int BN, bool flat_k = false) {
@@ -1073,7 +761,7 @@ bool encode_weights(CUtensorMap* mb, const void* w_split, int Cin, int taps, int
   if (flat_k) { cin_pad *= taps; taps = 1; }                     // K = tap * Cin + c as ONE dimension (taps are contiguous per Cout row)
   cuuint64_t dims[4] = {(cuuint64_t)cin_pad, (cuuint64_t)taps, (cuuint64_t)Cout, 2};
   cuuint64_t str[3] = {(cuuint64_t)cin_pad * 2, (cuuint64_t)taps * cin_pad * 2, (cuuint64_t)Cout * taps * cin_pad * 2};
-  cuuint32_t box[4] = {KE, 1, (cuuint32_t)(BN / 2), 1};          // each CTA of a pair loads (and multicasts) half of a plane's slab
+  cuuint32_t box[4] = {KE, 1, (cuuint32_t)(BN / 2), 1};          // a plane's BN-row slab is loaded as two half boxes
   return encode_map(mb, w_split, 4, dims, str, box, 1, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 }
 
@@ -1106,7 +794,7 @@ int tt_split_f16(const float* x, long long x_ld, void* y_split, long long y_plan
              "tt_split_f16", "needs 4-element alignment");
   if (rows == 0) return TT_OK;
   const long long total = rows * (cols / 4);
-  const int nb = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  const int nb = (int)((total + 255) / 256 > tt_num_sms() * 16 ? tt_num_sms() * 16 : (total + 255) / 256);
   split_rows_kernel<<<nb, 256, 0, (cudaStream_t)stream>>>(x, x_ld, static_cast<__half*>(y_split), y_plane, y_ld, rows, cols / 4, row_count);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_split_f16");
@@ -1120,7 +808,7 @@ int tt_image_to_split8(const float* x, void* y_split, long long y_plane, int N, 
              "tt_image_to_split8", "bad arguments");
   const long long total = (long long)N * H * W;
   if (total == 0) return TT_OK;
-  const int nb = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int nb = (int)((total + 255) / 256 > tt_num_sms() * 32 ? tt_num_sms() * 32 : (total + 255) / 256);
   image_to_split8_kernel<<<nb, 256, 0, (cudaStream_t)stream>>>(x, static_cast<__half*>(y_split), y_plane, C, H, W, out_H, out_W, top, left, total);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_image_to_split8");
@@ -1132,7 +820,7 @@ int tt_upsample2x_bilinear_ac_split(const float* x, void* y_split, long long y_p
              "tt_upsample2x_bilinear_ac_split", "C must be a multiple of 4, aligned pointers");
   const long long total = (long long)N * 4 * H * W * (C / 4);
   if (total == 0) return TT_OK;
-  const int nb = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int nb = (int)((total + 255) / 256 > tt_num_sms() * 32 ? tt_num_sms() * 32 : (total + 255) / 256);
   upsample2x_split_kernel<<<nb, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(x), static_cast<__half*>(y_split), y_plane, N, H, W, C / 4);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_upsample2x_bilinear_ac_split");
@@ -1155,7 +843,7 @@ int tt_pointwise_f16s(const tt_conv_desc* d, const tt_f16s_io* io, const float* 
   }
   const long long npix = (long long)d->N * d->H * d->W;
   if (npix == 0) return TT_OK;
-  const int nb = (int)((npix + 255) / 256 > 148 * 8 ? 148 * 8 : (npix + 255) / 256);
+  const int nb = (int)((npix + 255) / 256 > tt_num_sms() * 8 ? tt_num_sms() * 8 : (npix + 255) / 256);
   TT_REQUIRE(d->Cout % 8 == 0 || !io->y_split, "tt_pointwise_f16s", "plane output needs Cout % 8 == 0");
   const __half* xs = static_cast<const __half*>(io->x_split);
   __half* ys = static_cast<__half*>(io->y_split);
@@ -1181,7 +869,7 @@ int tt_merge_f16(const void* x_split, long long x_plane, long long x_ld, float* 
              "tt_merge_f16", "needs 4-element alignment");
   if (rows == 0) return TT_OK;
   const long long total = rows * (cols / 4);
-  const int nb = (int)((total + 255) / 256 > 148 * 16 ? 148 * 16 : (total + 255) / 256);
+  const int nb = (int)((total + 255) / 256 > tt_num_sms() * 16 ? tt_num_sms() * 16 : (total + 255) / 256);
   merge_rows_kernel<<<nb, 256, 0, (cudaStream_t)stream>>>(static_cast<const __half*>(x_split), x_plane, x_ld, y, y_ld, rows, cols / 4);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_merge_f16");
@@ -1256,21 +944,19 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
     if (!encode_map(&ma, x_split, 5, dims, str, box, d->stride, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return TT_ERR_CUDA;
     grid_x = a.tiles_w * a.tiles_h * d->N;
   }
-  const int BN = d->Cout > 64 ? 128 : 64;
   if (!encode_weights(&mb, w_split, d->Cin, taps, d->Cout, BN)) return TT_ERR_CUDA;
-  a.dbg = g_tt_debug & 0xFF;
   a.m_tiles = grid_x;
   a.n_tiles = tt_cdiv(d->Cout, BN);
-  const int num_sms = num_sms_cached();
+  const int num_sms = tt_num_sms();
   const int k_iters = taps * a.n_slabs;
   a.splits = 1;
   a.k_per = k_iters;
   {
-    const long long tile_pairs = (long long)((a.m_tiles + 1) / 2) * a.n_tiles;
+    const long long tiles = (long long)a.m_tiles * a.n_tiles;
     const bool plain = y != nullptr && d->oy_mul == 1 && d->ox_mul == 1 && d->oy_add == 0 && d->ox_add == 0 && d->yH == d->OH && d->yW == d->OW &&
                        d->res_mode != TT_RES_UP2_NEAREST && d->bias_n_mod == 0 && !(g_tt_debug & 128);
-    if (plain && tile_pairs * 2 <= num_sms / 2 && k_iters >= 8) {
-      int sp = (int)((num_sms / 2 + tile_pairs - 1) / tile_pairs);
+    if (plain && tiles <= num_sms / 2 && k_iters >= 8) {
+      int sp = (int)((num_sms + tiles - 1) / tiles);
       if (sp > k_iters / 4) sp = k_iters / 4;
       if (sp > 32) sp = 32;
       if (sp >= 2) {
@@ -1280,7 +966,7 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
     }
   }
   const long long total4 = (long long)d->N * d->OH * d->OW * (d->Cout / 4);
-  const int nb_ew = (int)((total4 + 255) / 256 > 1184 ? 1184 : (total4 + 255) / 256);
+  const int nb_ew = (int)((total4 + 255) / 256 > tt_num_sms() * 8 ? tt_num_sms() * 8 : (total4 + 255) / 256);
   if (a.splits > 1) {
     f16s_splitk_init_kernel<<<nb_ew, 256, 0, st>>>(*d, bias, d->res_mode != TT_RES_NONE ? res : nullptr, res2,
                                                    d->res_mode != TT_RES_NONE ? a.res_s : nullptr, a.res_plane, a.res2_s, a.res2_plane, y);
@@ -1290,21 +976,8 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
     a.d.act = TT_ACT_NONE;
     a.d.res_mode = TT_RES_NONE;
   }
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  // Correction accumulator drained once per work item (corr_once) where the TMEM drains set the pace and the extra N = BN
-  // instruction's operand reads do not: 1x1 layers with 2 .. 4 chunks per tile (K 256 .. 512).  Measured (profiles/r2_summary.md):
-  // 1x1 256->256 @112x224 +23 %; 3x3 256->256 -9 .. -18 % (shared-memory operand reads bound the long-K layers); one-chunk layers
-  // gain nothing.  Debug bits: 0x800000 forces it on everywhere, 0x1000000 off.
-  a.corr_once = (g_tt_debug & 0x1000000) ? 0 : ((g_tt_debug & 0x800000) || (taps == 1 && BN == 128 && a.splits == 1 && k_iters >= 4 && k_iters <= 8)) ? 1 : 0;
-  const cudaError_t lerr = BN == 128 ? launch_f16s<128, 3, 0>(cfg, ma, mb, a, a.m_tiles) : launch_f16s<64, 4, 0>(cfg, ma, mb, a, a.m_tiles);
-  if (lerr != cudaSuccess) { tt_set_error("tt_conv2d_f16s: cluster launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
+  const cudaError_t lerr = launch_f16s<0>(ma, mb, a, a.m_tiles, st);
+  if (lerr != cudaSuccess) { tt_set_error("tt_conv2d_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_conv2d_f16s");
   if (a.splits > 1 && (d->act != TT_ACT_NONE || y_split)) {
@@ -1329,7 +1002,7 @@ int tt_sparse_conv_f16s(const tt_sparse_conv_desc* d, const void* feats_in_split
   cudaStream_t st = (cudaStream_t)stream;
   if (d->cap_out <= 0) return TT_OK;
   const long long tot4 = (long long)d->cap_out * (d->Cout / 4);
-  const int nb = (int)((tot4 + 255) / 256 > 1184 ? 1184 : (tot4 + 255) / 256);
+  const int nb = (int)((tot4 + 255) / 256 > tt_num_sms() * 8 ? tt_num_sms() * 8 : (tot4 + 255) / 256);
   f16s_sparse_init_kernel<<<nb, 256, 0, st>>>(feats_out, d->out_ld, bias, d->Cout, out_count, d->cap_out);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_f16s(init)");
@@ -1342,28 +1015,17 @@ int tt_sparse_conv_f16s(const tt_sparse_conv_desc* d, const void* feats_in_split
   a.d.act = TT_ACT_NONE;
   a.y = feats_out;
   a.chunk = (g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2;
-  a.corr_once = (g_tt_debug & 0x800000) ? 1 : 0;
   a.n_slabs = (d->Cin + KE - 1) / KE;
-  a.dbg = g_tt_debug & 0xFF;
   a.gx = static_cast<const __half*>(feats_in_split); a.gx_plane = in_plane; a.gx_ld = d->in_ld;
   a.pairs_in = pairs_in; a.pairs_out = pairs_out; a.pair_count = pair_count;
   a.kvol = d->kvol; a.pair_cap = d->pair_cap;
   a.splits = 1; a.k_per = a.n_slabs;
-  const int BN = d->Cout > 64 ? 128 : 64;
   a.n_tiles = tt_cdiv(d->Cout, BN);
   CUtensorMap mb;
   if (!encode_weights(&mb, w_split, d->Cin, d->kvol, d->Cout, BN)) return TT_ERR_CUDA;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   const long long cap_units = (long long)d->kvol * tt_cdiv(d->pair_cap, BM);      // upper bound of gathered M tiles over all taps
-  const cudaError_t lerr = BN == 128 ? launch_f16s<128, 3, 1>(cfg, mb, mb, a, cap_units) : launch_f16s<64, 4, 1>(cfg, mb, mb, a, cap_units);
-  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_f16s: cluster launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
+  const cudaError_t lerr = launch_f16s<1>(mb, mb, a, cap_units, st);
+  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_f16s");
   f16s_sparse_finish_kernel<<<nb, 256, 0, st>>>(feats_out, d->out_ld, res, d->res_ld, d->Cout, out_count, d->cap_out, d->act,
@@ -1398,28 +1060,17 @@ int tt_sparse_conv_os_f16s(const tt_sparse_conv_desc* d, const tt_f16s_io* io, c
   a.res_s = static_cast<const __half*>(io->res_split); a.res_plane = io->res_plane;
   a.y = io->y; a.ys = static_cast<__half*>(io->y_split); a.ys_plane = io->y_plane;
   a.chunk = (g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2;
-  a.corr_once = (g_tt_debug & 0x800000) ? 1 : 0;
   a.n_slabs = (d->Cin + KE - 1) / KE;
-  a.dbg = g_tt_debug & 0xFF;
   a.gx = static_cast<const __half*>(io->x_split); a.gx_plane = io->x_plane; a.gx_ld = d->in_ld;
   a.kvol = d->kvol; a.nbr = nbr; a.out_count = out_count; a.cap_rows = d->cap_out;
   a.tps = (d->Cin == 32 && !(g_tt_debug & 0x200000)) ? 2 : 1;
   a.splits = 1; a.k_per = a.tps == 2 ? (d->kvol + 1) / 2 : d->kvol * a.n_slabs;
-  const int BN = d->Cout > 64 ? 128 : 64;
   a.n_tiles = tt_cdiv(d->Cout, BN);
   CUtensorMap mb;
   if (!encode_weights(&mb, io->w_split, d->Cin, d->kvol, d->Cout, BN, a.tps == 2)) return TT_ERR_CUDA;
-  cudaLaunchConfig_t cfg = {};
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.stream = (cudaStream_t)stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   const long long cap_units = tt_cdiv(d->cap_out, BM);
-  const cudaError_t lerr = BN == 128 ? launch_f16s<128, 3, 2>(cfg, mb, mb, a, cap_units) : launch_f16s<64, 4, 2>(cfg, mb, mb, a, cap_units);
-  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_os_f16s: cluster launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
+  const cudaError_t lerr = launch_f16s<2>(mb, mb, a, cap_units, (cudaStream_t)stream);
+  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_os_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_os_f16s");
   return TT_OK;

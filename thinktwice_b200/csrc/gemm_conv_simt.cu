@@ -379,7 +379,7 @@ __global__ void splitk_reduce_kernel(const ConvArgs p) {
 template <int BM, int BN, int TM, int TN>
 void launch_cfg(const ConvArgs& a, bool veca, bool vecb, cudaStream_t st) {
   int gx = tt_cdiv(a.M, BM);
-  if (a.m_count && gx > 148 * 8) gx = 148 * 8;                  // capacity-sized launches: grid-stride over the tiles
+  if (a.m_count && gx > tt_num_sms() * 8) gx = tt_num_sms() * 8;                  // capacity-sized launches: grid-stride over the tiles
   dim3 grid(gx, tt_cdiv(a.Cout_g, BN), a.d.groups * a.splits);
   if (veca && vecb) conv_igemm_simt<BM, BN, TM, TN, true, true><<<grid, 256, 0, st>>>(a);
   else if (veca) conv_igemm_simt<BM, BN, TM, TN, true, false><<<grid, 256, 0, st>>>(a);
@@ -430,7 +430,7 @@ int tt_conv2d_simt(const tt_conv_desc* d, const float* x, const float* w, const 
                     ((reinterpret_cast<uintptr_t>(y) & 15) == 0) &&
                     (res == nullptr || (reinterpret_cast<uintptr_t>(res) & 15) == 0) &&
                     (res2 == nullptr || (reinterpret_cast<uintptr_t>(res2) & 15) == 0);
-  // tile choice: big tiles when they still fill the 148 SMs, otherwise smaller ones
+  // tile choice: big tiles when they still fill the SMs, otherwise smaller ones
   const long long big = (long long)tt_cdiv(a.M, 128) * tt_cdiv(a.Cout_g, 128) * d->groups;
   if (a.splits > 1) {
     launch_cfg<64, 64, 4, 4>(a, veca, vecb, st);
@@ -442,8 +442,8 @@ int tt_conv2d_simt(const tt_conv_desc* d, const float* x, const float* w, const 
     TT_CHECK_LAUNCH("tt_conv2d(simt split-k reduce)");
     return TT_OK;
   }
-  if (a.Cout_g > 64 && big >= 148) launch_cfg<128, 128, 8, 8>(a, veca, vecb, st);
-  else if (a.Cout_g <= 64 && (long long)tt_cdiv(a.M, 128) * d->groups >= 148) launch_cfg<128, 64, 8, 4>(a, veca, vecb, st);
+  if (a.Cout_g > 64 && big >= tt_num_sms()) launch_cfg<128, 128, 8, 8>(a, veca, vecb, st);
+  else if (a.Cout_g <= 64 && (long long)tt_cdiv(a.M, 128) * d->groups >= tt_num_sms()) launch_cfg<128, 64, 8, 4>(a, veca, vecb, st);
   else launch_cfg<64, 64, 4, 4>(a, veca, vecb, st);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_conv2d(simt)");
@@ -506,7 +506,7 @@ extern "C" int tt_sparse_conv(const tt_sparse_conv_desc* d, const float* feats_i
   const bool vecb = (d->Cout % 4 == 0) && (d->out_ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(w) & 15) == 0) &&
                     ((reinterpret_cast<uintptr_t>(feats_out) & 15) == 0);
   TT_REQUIRE(d->kvol <= MAX_KVOL, "tt_sparse_conv", "kernel volume above 32 taps");
-  if (d->impl >= 2) {                                          // tcgen05 gather-GEMM; w = [2][Cout][kvol][Cin] hi / lo planes
+  if (d->impl >= 2) {                                          // tensor-core gather-GEMM; w = [2][Cout][kvol][Cin] hi / lo planes
     if (!tt_sparse_conv_tc_supported(d, feats_in, w, feats_out)) {
       tt_set_error("tt_sparse_conv: impl %d needs Cin, Cout >= 32 and multiples of 4, in_ld / out_ld multiples of 4, 16-byte aligned pointers", d->impl);
       return TT_ERR_UNSUPPORTED;
@@ -522,7 +522,7 @@ extern "C" int tt_sparse_conv(const tt_sparse_conv_desc* d, const float* feats_i
   a.accumulate = 2;
   {
     const long long cap_tiles = (long long)d->kvol * tt_cdiv(d->pair_cap, 64) * tt_cdiv(d->Cout, 64);
-    const int grid = (int)(cap_tiles < 148 * 6 ? cap_tiles : 148 * 6);
+    const int grid = (int)(cap_tiles < tt_num_sms() * 6 ? cap_tiles : tt_num_sms() * 6);
     if (veca && vecb) sparse_conv_taps_kernel<true, true><<<grid, 256, 0, st>>>(a, pairs_in, pairs_out, pair_count, d->kvol, d->pair_cap);
     else if (veca) sparse_conv_taps_kernel<true, false><<<grid, 256, 0, st>>>(a, pairs_in, pairs_out, pair_count, d->kvol, d->pair_cap);
     else if (vecb) sparse_conv_taps_kernel<false, true><<<grid, 256, 0, st>>>(a, pairs_in, pairs_out, pair_count, d->kvol, d->pair_cap);

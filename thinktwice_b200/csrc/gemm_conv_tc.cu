@@ -1,33 +1,29 @@
-// tcgen05 (5th-generation tensor core) implicit-GEMM convolution for sm_100a.
+// Hopper (sm_90a) implicit-GEMM convolution on the tensor cores (wgmma, TF32 operands).
 //
 // GEMM view: M = output pixels (one 128-row tile = a TH x TW rectangle of one image, or 128 consecutive
 // pixels for 1x1 convs), N = Cout (BN-wide tile), K = taps x Cin walked in 32-float (128-byte) slabs.
-//   * operands are staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a 3-stage shared-memory ring:
+//   * operands are staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a 4-stage shared-memory ring:
 //     the activation slab of tap (kh, kw) is ONE 4-D box load at a shifted origin — out-of-image pixels and
 //     channels are zero-filled by the TMA unit, so padding / dilation cost nothing;
-//   * one elected thread issues tcgen05.mma.cta_group::1.kind::tf32 (M128 x BN x K8) with the fp32
-//     accumulator tile living in TMEM (BN columns x 128 lanes);
+//   * two MMA warpgroups (rows 0..63 / 64..127 of the tile) issue wgmma.m64nNk8.f32.tf32.tf32 with the fp32
+//     accumulator tile in registers;
 //   * the raw fp32 activation slab is what TMA delivers; two "split" warps rewrite it in shared memory as hi (in place)
-//     and lo (second buffer) before the MMA thread may touch it — no pre-pass over the activations, no lo plane
-//     streamed from L2 (the kernel's roof is L2->SM ingest: profiles/r1_summary_tc.md);
+//     and lo (second buffer) before the MMA warpgroups may touch it — no pre-pass over the activations, no lo plane
+//     streamed from L2;
 //   * precision: fp32 operands are split x = hi + lo (activations: hi = RN_tf32(x), lo = x - hi, split in shared
 //     memory; weights: hi / lo planes prepared once on the host) and every K slab issues hi*hi + hi*lo + lo*hi
-//     ("3xTF32": ~21 mantissa bits per operand) as TWO instructions: A_hi x [B_hi ; B_lo] with N = 2 BN (the lo weight
-//     tile follows the hi tile in shared memory, the correction accumulator follows the main one in TMEM) and
-//     A_lo x B_hi.  The tensor core adds into its fp32 accumulator with truncation, an error that grows linearly with
-//     the number of accumulations (measured: ~8e-9 * K relative), so (a) the two small correction products have their
-//     OWN TMEM accumulator and (b) every CHUNK K-slabs the epilogue warps drain both accumulators with tcgen05.ld and
-//     fold them into fp32 registers with round-to-nearest FADDs while the MMA warp already fills the other accumulator
-//     pair (TMEM ping-pong: 2 x (main + corr) x BN columns = all 512 columns at BN = 128).  impl == TF32x1: hi*hi only;
-//   * epilogue: 8 warps (two per TMEM lane quarter) read the accumulators with tcgen05.ld, transpose through warp-
-//     private shared-memory slabs and store coalesced channels-last rows with bias + residual(s) + activation fused
-//     (concat offset / pixel scatter for transposed convs handled in the store address);
-//   * persistent CTA pairs (cluster of 2): both CTAs walk the same (M-tile pair, N tile) list, each loads half of the
-//     weight slab and TMA-multicasts it to its peer;
+//     ("3xTF32": ~21 mantissa bits per operand) as three m64nBNk8 instructions into two register arrays: main += A_hi x B_hi,
+//     corr += A_hi x B_lo + A_lo x B_hi (one shape for all of them: wgmma of different shapes on overlapping accumulators
+//     would be serialised by the compiler).  The tensor core adds into its fp32 accumulator with truncation, an error that grows
+//     linearly with the number of accumulations, so every CHUNK K-slabs the register accumulator is restarted and folded
+//     into fp32 sums with round-to-nearest FADDs.  impl == TF32x1: hi*hi only;
+//   * epilogue: each MMA warp transposes its 16 accumulator rows through a warp-private shared-memory slab and stores
+//     coalesced channels-last rows with bias + residual(s) + activation fused (concat offset / pixel scatter for
+//     transposed convs handled in the store address);
+//   * persistent CTAs (one per SM) walk the (M tile, N tile, K split) list;
 //   * split-K for under-filled layers (few tiles, long K) and GATHER mode (tap-major sparse convolution: cp.async row
 //     gather) both end in a red.add.v4.f32 epilogue into a pre-initialised output.
-// Warp roles: warp 0 = TMA / gather producer, warp 1 = TMEM allocator + MMA issuer, warps 2..9 = epilogue,
-// warps 10..11 = operand split.
+// Warp roles: warp 0 = TMA / gather producer, warp 1 idle, warps 2..3 = operand split, warps 4..11 = MMA + epilogue.
 #include <cuda.h>
 #include <string.h>
 
@@ -39,13 +35,13 @@ extern int g_tt_debug;
 
 namespace {
 
-constexpr int BM = 128;          // UMMA M
-constexpr int KS = 32;           // floats per K slab (one 128-byte swizzle row)
-constexpr int NTHREADS = 384;     // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter), warps 10..11 operand split
+constexpr int BM = 128;           // M tile: two warpgroups x 64 rows
+constexpr int KS = 32;            // floats per K slab (one 128-byte swizzle row)
+constexpr int NTHREADS = 384;     // warpgroup 0: producer + split warps; warpgroups 1..2: MMA + epilogue
+// N tile: 3xTF32 holds BN fp32 accumulators (main | corr) plus BN / 2 fp32 sums per MMA thread, within the compiler's
+// 168-register budget at 384 threads only for BN = 64
+constexpr int BN = 64, STAGES = 4;
 
-// ------------------------------------------------------------------------------------------------ PTX helpers
-// (PTX wrappers: tc_ptx.cuh)
-// ------------------------------------------------------------------------------------------------ kernels
 struct TcArgs {
   tt_conv_desc d;
   const float* bias;
@@ -56,10 +52,8 @@ struct TcArgs {
   int tiles_w, tiles_h;  // tiles per image along W and H
   int flat;              // 1: 1x1 conv on the flattened pixel axis
   int n_slabs;           // ceil(Cin / 32)
-  int terms;             // 3: hi*hi + hi*lo + lo*hi ; 1: hi*hi only
-  int chunk;             // K slabs accumulated inside TMEM before the epilogue folds them into fp32 registers
+  int chunk;             // K slabs accumulated by the tensor core before the MMA warps fold them into fp32 sums
   int total_pix;         // N * OH * OW
-  int dbg;               // diagnosis knobs (tt_debug_set): 1 = no epilogue global traffic, 2 = no A loads, 4 = no MMAs
   int m_tiles, n_tiles;  // persistent tile walk: tile t -> (m tile t / n_tiles, n tile t % n_tiles)
   // GATHER (tap-major sparse convolution): GEMM rows are the (input row, output row) pairs of one kernel tap
   const float* gx;       // feature rows [.][gx_ld]
@@ -68,7 +62,7 @@ struct TcArgs {
   const int* pairs_out;  // [kvol][pair_cap]
   const int* pair_count; // [kvol]
   int kvol, pair_cap;
-  // split-K (under-filled layers: few tiles, long K): work item = (tile pair, N tile, K split); partial sums are
+  // split-K (under-filled layers: few tiles, long K): work item = (tile, N tile, K split); partial sums are
   // red.add-ed into an output the host pre-initialised with bias + residuals, activation applied by a finish kernel
   int splits, k_per;     // K slabs per split (k_per * splits >= taps * n_slabs)
 };
@@ -76,25 +70,21 @@ constexpr int MAX_KVOL = 32;
 
 // operand split used by the in-kernel split warps: hi = x rounded to nearest TF32 (ties away: one IADD + one LOP3 on
 // the alu pipe), lo = x - hi (exact in fp32, one FADD on the fma pipe).  |lo| <= 2^-11 |x| with either sign, so the
-// tensor core's own fp32 -> tf32 truncation of lo is an unbiased 2^-21-relative perturbation.  Anything heavier makes the
-// two split warps the bottleneck: the alu pipe issues one warp instruction per 2 clocks per SM sub-partition.
+// tensor core's own fp32 -> tf32 truncation of lo is an unbiased 2^-21-relative perturbation.
 TT_DEVICE void split_rn(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
   lo = x - hi;
 }
 
-// CTA PAIRS (thread-block cluster of 2, one TPC): the two CTAs work on two different M tiles of the SAME N tile in
-// lockstep; each loads half of the weight slab and TMA-multicasts it into both CTAs' shared memory, halving the
-// weight traffic from L2 (the kernel's measured roof is L2->SM bandwidth).  A stage is refilled only after BOTH
-// MMA threads released it (multicast tcgen05.commit onto both CTAs' `empty` barriers, count 2).
-// Persistent, warp-specialised kernel: each CTA pair walks tile pairs pt = blockIdx.x / 2, += gridDim.x / 2.  The smem
-// ring, the TMEM ping-pong and all phase counters run ACROSS tiles, so while the epilogue warps store tile i the
-// TMA and MMA warps are already deep into tile i + 1.
+// Persistent, warp-specialised kernel: each CTA walks work items pt = blockIdx.x, += gridDim.x.  The smem ring and all
+// phase counters run ACROSS tiles, so while the MMA warps store tile i the TMA warp is already loading tile i + 1.
 // GATHER = true turns the kernel into the tap-major sparse convolution (spconv SubMConv3d / SparseConv3d): work items
-// are (tap, pair-tile pair, N tile); warp 0 gathers the activation rows of a tile with 16-byte cp.async (zero-fill for
+// are (tap, pair tile, N tile); warp 0 gathers the activation rows of a tile with 16-byte cp.async (zero-fill for
 // the tile tail / channel tail) straight into the 128-byte-swizzled stage buffer, signalling the same `full` barrier
 // the weight TMA uses; the epilogue accumulates into the bias-initialised output rows with red.add.v4.f32.
-template <int BN, int STAGES, bool GATHER>
+// TERMS: 3 = 3xTF32 (hi*hi + hi*lo + lo*hi), 1 = single-pass TF32 (hi*hi only); a template parameter so that the MMA loop has no
+// run-time branch between wgmma instructions.
+template <int TERMS, bool GATHER>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b_hi,
                const __grid_constant__ CUtensorMap map_b_lo, const TcArgs p) {
@@ -102,64 +92,40 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   constexpr int A_BYTES = BM * KS * 4;                    // 16 KB
   constexpr int B_BYTES = BN * KS * 4;
   constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  // TMEM: 2 (ping-pong) x {main, corr} x BN fp32 columns (all 512 columns at BN = 128)
-  constexpr int ACC_COLS = 2 * BN;
-  constexpr int TMEM_COLS = 2 * ACC_COLS;
-  constexpr int SLAB = 16;                                // epilogue slab: 16 columns of a warp's 32 rows
+  constexpr int SLAB = 16;                                // epilogue column slab
   constexpr int PITCH = SLAB + 4;                         // +4 floats: conflict-free transposition
-  constexpr int HN = BN / 2;                              // columns owned by one epilogue warp (column half)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* tile_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);              // [8 warps][32 rows][PITCH]
-  long long* row_y = reinterpret_cast<long long*>(tile_all + 8 * 32 * PITCH);                   // [128] output offset of row
-  long long* row_r1 = row_y + BM;                                                       // [128] residual-1 pixel
-  long long* row_r2 = row_r1 + BM;                                                      // [128] residual-2 pixel (= GEMM row)
-  int* row_flag = reinterpret_cast<int*>(row_r2 + BM);                                  // [128] valid | image << 1
-  uint64_t* bars = reinterpret_cast<uint64_t*>(row_flag + BM);
+  float* tile_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);              // [8 MMA warps][16 rows][PITCH]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tile_all + 8 * 16 * PITCH);
   uint64_t* full = bars;                                  // [STAGES]  TMA -> split warps (raw operands landed)
-  uint64_t* empty = bars + STAGES;                        // [STAGES]  MMA -> TMA
+  uint64_t* empty = bars + STAGES;                        // [STAGES]  MMA warps -> TMA
   uint64_t* conv = bars + 2 * STAGES;                     // [STAGES]  split warps -> MMA (hi / lo written)
-  uint64_t* acc_full = bars + 3 * STAGES;                 // [2]       MMA -> epilogue (chunk finished)
-  uint64_t* acc_empty = bars + 3 * STAGES + 2;            // [2]       epilogue -> MMA (accumulators drained)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * STAGES + 4);
-  int* sp_first = reinterpret_cast<int*>(tmem_slot + 2);   // GATHER: [kvol + 1] first tile pair of each tap
+  int* sp_first = reinterpret_cast<int*>(bars + 3 * STAGES);   // GATHER: [kvol + 1] first tile of each tap
   int* sp_cnt = sp_first + MAX_KVOL + 1;                  // GATHER: [kvol] pairs of each tap
 
   const tt_conv_desc& d = p.d;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int taps = d.KH * d.KW;
   const int k_iters = taps * p.n_slabs;
-  const uint32_t rank = cluster_ctarank();                // 0 / 1 inside the CTA pair
-  const int pair0 = blockIdx.x >> 1, pair_step = gridDim.x >> 1;
 
   if (threadIdx.x == 0) {
-    // full: the producer's expect_tx arrival (+ 32 cp.async arrivals in GATHER mode); empty: both MMA threads of the pair;
-    // conv: 2 split warps
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GATHER ? 33 : 1); mbar_init(&empty[s], 2); mbar_init(&conv[s], 2); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 8); }   // 8 epilogue warps arrive
+    // full: the producer's expect_tx arrival (+ 32 cp.async arrivals in GATHER mode); empty: the 8 MMA warps; conv: 2 split warps
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GATHER ? 33 : 1); mbar_init(&empty[s], 8); mbar_init(&conv[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (GATHER && threadIdx.x == 64) {                        // tile-pair prefix over the taps (identical in both CTAs)
+  if (GATHER && threadIdx.x == 64) {                        // tile prefix over the taps
     int acc = 0;
     for (int t = 0; t < p.kvol; ++t) {
       const int c = min(p.pair_count[t], p.pair_cap);
       sp_cnt[t] = c;
       sp_first[t] = acc;
-      acc += ((c + BM - 1) / BM + 1) / 2;
+      acc += (c + BM - 1) / BM;
     }
     sp_first[p.kvol] = acc;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  cluster_sync_all();                                       // the peer's barriers are initialised before any multicast lands
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // both CTAs iterate the same pair list (lockstep)
-  const int total_pairs = (GATHER ? sp_first[p.kvol] : (p.m_tiles + 1) / 2) * p.n_tiles * p.splits;
-  // work item -> (N tile, M tile of this CTA, tap, rows of that tap)
+  const int total_items = (GATHER ? sp_first[p.kvol] : p.m_tiles) * p.n_tiles * p.splits;
+  // work item -> (N tile, M tile, tap, rows of that tap)
   auto decode = [&](int pt, int& nt, int& mt, int& tap, int& count, int& kb, int& ke) {
     const int ks = pt % p.splits;
     pt /= p.splits;
@@ -170,61 +136,67 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     tap = 0; count = 0;
     if (GATHER) {
       while (sp_first[tap + 1] <= pm) ++tap;
-      mt = 2 * (pm - sp_first[tap]) + (int)rank;
+      mt = pm - sp_first[tap];
       count = sp_cnt[tap];
     } else {
-      mt = 2 * pm + (int)rank;
+      mt = pm;
+    }
+  };
+  // weight slab of one stage: hi plane (+ lo plane), BN rows each, loaded as two BN / 2-row boxes per plane
+  auto load_weights = [&](uint8_t* st, uint64_t* bar, int k0, int tap, int n0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      tma_load_3d(st + 2 * A_BYTES + h * (B_BYTES / 2), &map_b_hi, bar, k0, tap, n0 + h * (BN / 2));
+      if (TERMS == 3) tma_load_3d(st + 2 * A_BYTES + B_BYTES + h * (B_BYTES / 2), &map_b_lo, bar, k0, tap, n0 + h * (BN / 2));
     }
   };
 
-  if (warp == 0 && GATHER) {
-    // ===================================================================== gather producer (whole warp) + weight TMA
-    const uint32_t txb = (p.terms == 3 ? 2 : 1) * B_BYTES;
-    int ig = 0;
-    for (int pt = pair0; pt < total_pairs; pt += pair_step) {
-      int nt, mt, tap, count, kb, ke;
-      decode(pt, nt, mt, tap, count, kb, ke);
-      const int n0 = nt * BN;
-      const int* pin = p.pairs_in + (long long)tap * p.pair_cap;
-      int rows[4];                                            // this lane's rows: lane, lane + 32, lane + 64, lane + 96
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int m = mt * BM + lane + 32 * i;
-        rows[i] = m < count ? __ldg(pin + m) : -1;
-      }
-      for (int it = kb; it < ke; ++it, ++ig) {
-        const int s = ig % STAGES;
-        mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
-        uint8_t* st = smem + s * STAGE_BYTES;
-        if (lane == 0) {
-          mbar_expect_tx(&full[s], txb);
-          tma_load_3d_mc(st + 2 * A_BYTES + rank * (B_BYTES / 2), &map_b_hi, &full[s], it * KS, tap, n0 + (int)rank * (BN / 2), 3);
-          if (p.terms == 3)
-            tma_load_3d_mc(st + 2 * A_BYTES + B_BYTES + rank * (B_BYTES / 2), &map_b_lo, &full[s], it * KS, tap, n0 + (int)rank * (BN / 2), 3);
-        }
-        const int c0 = it * KS;
+  if (warp < 4) {
+    if (warp == 0 && GATHER) {
+      // ===================================================================== gather producer (whole warp) + weight TMA
+      const uint32_t txb = (TERMS == 3 ? 2 : 1) * B_BYTES;
+      int ig = 0;
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
+        int nt, mt, tap, count, kb, ke;
+        decode(pt, nt, mt, tap, count, kb, ke);
+        const int n0 = nt * BN;
+        const int* pin = p.pairs_in + (long long)tap * p.pair_cap;
+        int rows[4];                                            // this lane's rows: lane, lane + 32, lane + 64, lane + 96
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const int r = lane + 32 * i;
-          const float* src = p.gx + (long long)max(rows[i], 0) * p.gx_ld + c0;
-          const uint32_t dst = smem_u32(st) + r * 128;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {                       // 16-byte chunk j of row r lives at chunk j ^ (r & 7)
-            const bool ok = rows[i] >= 0 && c0 + j * 4 < d.Cin;
-            cp_async16(dst + ((j ^ (r & 7)) << 4), ok ? src + j * 4 : p.gx, ok ? 16 : 0);
-          }
+          const int m = mt * BM + lane + 32 * i;
+          rows[i] = m < count ? __ldg(pin + m) : -1;
         }
-        cp_async_arrive_noinc(&full[s]);
+        for (int it = kb; it < ke; ++it, ++ig) {
+          const int s = ig % STAGES;
+          mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
+          uint8_t* st = smem + s * STAGE_BYTES;
+          if (lane == 0) {
+            mbar_expect_tx(&full[s], txb);
+            load_weights(st, &full[s], it * KS, tap, n0);
+          }
+          const int c0 = it * KS;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int r = lane + 32 * i;
+            const float* src = p.gx + (long long)max(rows[i], 0) * p.gx_ld + c0;
+            const uint32_t dst = smem_u32(st) + r * 128;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {                       // 16-byte chunk j of row r lives at chunk j ^ (r & 7)
+              const bool ok = rows[i] >= 0 && c0 + j * 4 < d.Cin;
+              cp_async16(dst + ((j ^ (r & 7)) << 4), ok ? src + j * 4 : p.gx, ok ? 16 : 0);
+            }
+          }
+          cp_async_arrive_noinc(&full[s]);
+        }
       }
-    }
-  } else if (warp == 0) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
+    } else if (warp == 0 && lane == 0) {
+      // ===================================================================== TMA producer
       const uint32_t a_box = (uint32_t)(p.flat ? BM : p.TH * p.TW) * KS * 4;   // bytes one activation box delivers
-      const uint32_t tx = ((p.dbg & 2) ? 0u : a_box) + (p.terms == 3 ? 2 : 1) * B_BYTES;     // own raw A + both weight halves
+      const uint32_t tx = a_box + (TERMS == 3 ? 2 : 1) * B_BYTES;
       int ig = 0;                                                               // ring position, continues across tiles
-      for (int pt = pair0; pt < total_pairs; pt += pair_step) {
-        int nt, mt, tap0, count, kb, ke;                                        // mt >= m_tiles: dummy tile, TMA zero-fills
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
+        int nt, mt, tap0, count, kb, ke;
         decode(pt, nt, mt, tap0, count, kb, ke);
         const int n0 = nt * BN;
         int cw0, ch0, cn;
@@ -242,249 +214,186 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
           const int kh = tap / d.KW, kw = tap - kh * d.KW;
           mbar_expect_tx(&full[s], tx);
           const int cw = p.flat ? cw0 : cw0 + kw * d.dil, ch = p.flat ? 0 : ch0 + kh * d.dil;
-          if (!(p.dbg & 2)) tma_load_4d(st, &map_a, &full[s], slab * KS, cw, ch, cn);      // raw fp32 activations
-          tma_load_3d_mc(st + 2 * A_BYTES + rank * (B_BYTES / 2), &map_b_hi, &full[s], slab * KS, tap, n0 + (int)rank * (BN / 2), 3);
-          if (p.terms == 3) {
-            tma_load_3d_mc(st + 2 * A_BYTES + B_BYTES + rank * (B_BYTES / 2), &map_b_lo, &full[s], slab * KS, tap, n0 + (int)rank * (BN / 2), 3);
-          }
+          tma_load_4d(st, &map_a, &full[s], slab * KS, cw, ch, cn);      // raw fp32 activations
+          load_weights(st, &full[s], slab * KS, tap, n0);
         }
       }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== MMA issuer (one thread)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BM, BN);
-      constexpr uint32_t idesc2 = make_idesc(BM, 2 * BN);                 // hi*hi | hi*lo in one instruction
-      int ig = 0, cg = 0;                                                       // ring / chunk counters across tiles
-      for (int pt = pair0; pt < total_pairs; pt += pair_step) {
+    } else if (warp >= 2) {
+      // ===================================================================== operand split (warps 2, 3)
+      // Each warp owns 64 rows of the 128 x 32-float activation slab: raw -> hi in place, lo into the second buffer.
+      // Element-wise at identical offsets, so the 128-byte swizzle TMA applied is irrelevant here.
+      const int w2 = warp - 2;
+      int ig = 0;
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
         int nt, mt, tap0, count, kb, ke;
         decode(pt, nt, mt, tap0, count, kb, ke);
-        int it = kb;
-        const int nch = (ke - kb + p.chunk - 1) / p.chunk;
-        for (int c = 0; c < nch; ++c, ++cg) {
-          const int b = cg & 1;
-          mbar_wait(&acc_empty[b], ((cg >> 1) & 1) ^ 1);     // epilogue has drained this accumulator pair
-          tcgen05_fence_after();
-          const uint32_t t_main = tmem_base + (uint32_t)(b * ACC_COLS), t_corr = t_main + BN;
-          const int it_end = min(it + p.chunk, ke);
-          bool first = true;
-          for (; it < it_end; ++it, ++ig) {
-            const int s = ig % STAGES;
-            mbar_wait(&conv[s], (ig / STAGES) & 1);         // operands landed AND split into hi / lo
-            tcgen05_fence_after();
-            const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES), a_lo = a_hi + A_BYTES;
-            const uint32_t b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+        for (int it = kb; it < ke; ++it, ++ig) {
+          const int s = ig % STAGES;
+          mbar_wait(&full[s], (ig / STAGES) & 1);
+          const uint32_t raw = smem_u32(smem + s * STAGE_BYTES) + w2 * (A_BYTES / 2) + lane * 16;   // lo at + A_BYTES
+          // all loads of a batch are issued before any store: the loop is latency-bound otherwise
 #pragma unroll
-            for (int kk = 0; kk < KS / 8; ++kk) {            // UMMA K = 8 tf32 = 32 bytes inside the 128-byte swizzle row
-              if (p.dbg & 4) break;
-              const uint32_t off = kk * 32;
-              const uint32_t acc = (first && kk == 0) ? 0u : 1u;
-              if (p.terms == 3 && !(p.dbg & 32)) {
-                // A_hi x [B_hi ; B_lo] as ONE N = 2 BN instruction: the lo weight tile follows the hi tile in shared
-                // memory and the correction accumulator follows the main one in TMEM, so hi*hi and hi*lo share a
-                // single read of the A_hi slab (the tf32 SS-MMA rate is shared-memory-read bound).
-                umma_tf32(t_main, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), idesc2, acc);
-                umma_tf32(t_corr, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), idesc, 1);
-              } else {
-                umma_tf32(t_main, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), idesc, acc);
-                if (p.terms == 3) {
-                  umma_tf32(t_corr, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), idesc, acc);
-                  umma_tf32(t_corr, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), idesc, 1);
-                }
-              }
+          for (int b0 = 0; b0 < A_BYTES / 32 / 32; b0 += 8) {    // 16 float4 per lane, two batches of 8
+            float4 v[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) v[u] = lds128(raw + (b0 + u) * 512);
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+              float4 h, l;
+              split_rn(v[u].x, h.x, l.x); split_rn(v[u].y, h.y, l.y); split_rn(v[u].z, h.z, l.z); split_rn(v[u].w, h.w, l.w);
+              sts128(raw + (b0 + u) * 512, h);
+              if (TERMS == 3) sts128(raw + A_BYTES + (b0 + u) * 512, l);
             }
-            first = false;
-            tcgen05_commit_mc(&empty[s], 3);                 // releases the slot in BOTH CTAs once these MMAs retire
           }
-          tcgen05_commit(&acc_full[b]);                      // chunk complete -> epilogue may drain
+          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+          __syncwarp();
+          if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&conv[s])) : "memory");
         }
-      }
-    }
-  } else if (warp >= 10) {
-    // ===================================================================== operand split (warps 10, 11)
-    // Each warp owns 64 rows of the 128 x 32-float activation slab: raw -> hi in place, lo into the second buffer.
-    // Element-wise at identical offsets, so the 128-byte swizzle TMA applied is irrelevant here.
-    const int w2 = warp - 10;
-    int ig = 0;
-    for (int pt = pair0; pt < total_pairs; pt += pair_step) {
-      int nt, mt, tap0, count, kb, ke;
-      decode(pt, nt, mt, tap0, count, kb, ke);
-      for (int it = kb; it < ke; ++it, ++ig) {
-        const int s = ig % STAGES;
-        mbar_wait(&full[s], (ig / STAGES) & 1);
-        const uint32_t raw = smem_u32(smem + s * STAGE_BYTES) + w2 * (A_BYTES / 2) + lane * 16;   // lo at + A_BYTES
-        // all loads of a batch are issued before any store: the loop is latency-bound otherwise (16 dependent
-        // ld -> alu -> st round trips per stage per lane)
-#pragma unroll
-        for (int b0 = 0; b0 < A_BYTES / 32 / 32; b0 += 8) {    // 16 float4 per lane, two batches of 8
-          float4 v[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) v[u] = lds128(raw + (b0 + u) * 512);
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            float4 h, l;
-            split_rn(v[u].x, h.x, l.x); split_rn(v[u].y, h.y, l.y); split_rn(v[u].z, h.z, l.z); split_rn(v[u].w, h.w, l.w);
-            if (p.dbg & 64) {                                  // experiment: lo rounded to nearest TF32 instead of truncated by the MMA
-              float t;
-              split_rn(l.x, l.x, t); split_rn(l.y, l.y, t); split_rn(l.z, l.z, t); split_rn(l.w, l.w, t);
-            }
-            sts128(raw + (b0 + u) * 512, h);
-            if (p.terms == 3) sts128(raw + A_BYTES + (b0 + u) * 512, l);
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&conv[s])) : "memory");
       }
     }
   } else {
-    // ===================================================================== epilogue (warps 2..9)
-    const int q = warp & 3;                                // this warp may touch TMEM lanes [32q, 32q + 32)
-    const int half = (warp - 2) >> 2;                      // and owns columns [half * HN, half * HN + HN) of the tile
-    const int r = q * 32 + lane;                           // accumulator row = pixel within the tile
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
+    // ===================================================================== MMA + epilogue (warpgroups 1, 2)
+    const int cw = warp - 4;                                // MMA warp 0..7
+    const int wg = cw >> 2;                                 // warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int row0 = wg * 64 + (cw & 3) * 16;               // this warp's 16 accumulator rows
     const long long yns = d.y_nstride ? d.y_nstride : (long long)d.yH * d.yW * d.y_ld;
     const int HWo = d.OH * d.OW;
-    float* tile = tile_all + (warp - 2) * 32 * PITCH;      // warp-private transposition buffer [32 rows][PITCH]
-    int cg = 0;
-    for (int pt = pair0; pt < total_pairs; pt += pair_step) {
+    float* tile = tile_all + cw * 16 * PITCH;               // warp-private transposition buffer [16 rows][PITCH]
+    const int sub = lane >> 2, cl = (lane & 3) * 4;         // store phase: 4 lanes per row, 8 rows per warp instruction
+    int ig = 0;
+    for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
       int nt, mt, tap, count, kb, ke;
       decode(pt, nt, mt, tap, count, kb, ke);
       const int nch = (ke - kb + p.chunk - 1) / p.chunk;
       const bool real_tile = GATHER ? mt * BM < count : mt < p.m_tiles;
-      const int n0 = nt * BN + half * HN;
-      // ---- this thread's row -> output / residual addresses (once per tile); prefetch the residual lines into L2
-      if (GATHER) {
-        const int m = mt * BM + r;
-        const bool valid = m < count;
-        if (half == 0) {
+      const int n0 = nt * BN;
+      // ---- output / residual addresses of the two rows this lane stores (rows row0 + sub, row0 + 8 + sub)
+      int fl[2];
+      long long yo[2], o1[2], o2[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int r = row0 + i * 8 + sub;
+        if (GATHER) {
+          const int m = mt * BM + r;
+          const bool valid = m < count;
           const int orow = valid ? __ldg(p.pairs_out + (long long)tap * p.pair_cap + m) : 0;
-          row_y[r] = (long long)orow * d.y_ld + d.y_coff;
-          row_r1[r] = 0;
-          row_r2[r] = 0;
-          row_flag[r] = valid ? 1 : 0;
-        }
-      } else {
-        bool valid;
-        int nimg, oh, ow;
-        long long rrow;
-        if (p.flat) {
-          const long long pix = (long long)mt * BM + r;
-          valid = real_tile && pix < p.total_pix;
-          nimg = (int)(pix / HWo);
-          const int rem = (int)(pix - (long long)nimg * HWo);
-          oh = rem / d.OW; ow = rem - oh * d.OW;
-          rrow = pix;
+          yo[i] = (long long)orow * d.y_ld + d.y_coff;
+          o1[i] = 0; o2[i] = 0;
+          fl[i] = valid ? 1 : 0;
         } else {
-          const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h;
-          nimg = mt / (p.tiles_w * p.tiles_h);
-          const int rh = r / p.TW, rw = r - rh * p.TW;
-          oh = th * p.TH + rh; ow = tw * p.TW + rw;
-          valid = real_tile && (r < p.TH * p.TW) && oh < d.OH && ow < d.OW;
-          rrow = ((long long)nimg * d.OH + oh) * d.OW + ow;
-        }
-        const long long r1 = (d.res_mode == TT_RES_UP2_NEAREST
-                                  ? ((long long)nimg * d.res_H + (oh * d.res_H) / d.OH) * d.res_W + (ow * d.res_W) / d.OW
-                                  : rrow) * d.res_ld + d.res_coff;
-        const long long r2 = rrow * d.res2_ld + d.res2_coff;
-        if (half == 0) {                                    // both column halves would write identical values
-          row_y[r] = nimg * yns + ((long long)(oh * d.oy_mul + d.oy_add) * d.yW + ow * d.ox_mul + d.ox_add) * d.y_ld + d.y_coff;
-          row_r1[r] = r1;
-          row_r2[r] = r2;
-          row_flag[r] = (valid ? 1 : 0) | (nimg << 1);
-        }
-        if (valid && n0 < d.Cout) {
-          if (p.res) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res + r1 + n0 + j));
-          }
-          if (p.res2) {
-#pragma unroll
-            for (int j = 0; j < HN; j += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.res2 + r2 + n0 + j));
-          }
-        }
-      }
-      float sum[HN];
-#pragma unroll
-      for (int j = 0; j < HN; ++j) sum[j] = 0.f;
-      for (int c = 0; c < nch; ++c, ++cg) {
-        const int b = cg & 1;
-        mbar_wait(&acc_full[b], (cg >> 1) & 1);
-        tcgen05_fence_after();
-        const uint32_t t_main = tmem_base + lane_addr + (uint32_t)(b * ACC_COLS + half * HN);
-#pragma unroll
-        for (int c0 = 0; c0 < HN; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(t_main + c0, v);
-          if (p.terms == 3) {
-            uint32_t u[32];
-            tmem_ld32(t_main + BN + c0, u);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) sum[c0 + j] += __uint_as_float(v[j]) + __uint_as_float(u[j]);   // fp32 RN adds
+          bool valid;
+          int nimg, oh, ow;
+          long long rrow;
+          if (p.flat) {
+            const long long pix = (long long)mt * BM + r;
+            valid = real_tile && pix < p.total_pix;
+            nimg = (int)(pix / HWo);
+            const int rem = (int)(pix - (long long)nimg * HWo);
+            oh = rem / d.OW; ow = rem - oh * d.OW;
+            rrow = pix;
           } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) sum[c0 + j] += __uint_as_float(v[j]);
+            const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h;
+            nimg = mt / (p.tiles_w * p.tiles_h);
+            const int rh = r / p.TW, rw = r - rh * p.TW;
+            oh = th * p.TH + rh; ow = tw * p.TW + rw;
+            valid = real_tile && (r < p.TH * p.TW) && oh < d.OH && ow < d.OW;
+            rrow = ((long long)nimg * d.OH + oh) * d.OW + ow;
           }
+          o1[i] = (d.res_mode == TT_RES_UP2_NEAREST
+                       ? ((long long)nimg * d.res_H + (oh * d.res_H) / d.OH) * d.res_W + (ow * d.res_W) / d.OW
+                       : rrow) * d.res_ld + d.res_coff;
+          o2[i] = rrow * d.res2_ld + d.res2_coff;
+          yo[i] = nimg * yns + ((long long)(oh * d.oy_mul + d.oy_add) * d.yW + ow * d.ox_mul + d.ox_add) * d.y_ld + d.y_coff;
+          fl[i] = (valid ? 1 : 0) | (nimg << 1);
         }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&acc_empty[b])) : "memory");
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");         // row tables written by the half-0 warps are visible
-      // ---- coalesced store in 16-column slabs: registers -> smem (transpose) -> 64-byte row segments, 8 rows / instr
-      const int sub = lane >> 2, cl = (lane & 3) * 4;        // 4 lanes per row, 8 rows per warp instruction
+      // ---- K walk: chunks of `chunk` slabs accumulated by the tensor core, folded into fp32 sums with RN adds
+      float sum[BN / 2];
 #pragma unroll
-      for (int sl = 0; sl < HN / SLAB; ++sl) {
+      for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
+      auto release = [&](int s) {                            // this warp's wgmmas no longer read stage s
+        __syncwarp();
+        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
+      };
+      int it = kb;
+      for (int c = 0; c < nch; ++c) {
+        float acc[BN / 2], cor[BN / 2];                      // main and correction accumulators
+        const int it_end = min(it + p.chunk, ke);
+        int held = -1;                                       // the stage whose wgmmas may still be in flight
+        for (bool first = true; it < it_end; ++it, ++ig, first = false) {
+          const int s = ig % STAGES;
+          mbar_wait(&conv[s], (ig / STAGES) & 1);           // operands landed AND split into hi / lo
+          const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES) + wg * (A_BYTES / 2), a_lo = a_hi + A_BYTES;
+          const uint32_t b_hi = smem_u32(smem + s * STAGE_BYTES) + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < KS / 8; ++kk) {              // K = 8 tf32 = 32 bytes inside the 128-byte swizzle row
+            const uint32_t off = kk * 32, z = (first && kk == 0) ? 0u : 1u;
+            wgmma_tf32<BN>(acc, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), z);          // hi*hi
+            if constexpr (TERMS == 3) {
+              wgmma_tf32<BN>(cor, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), z);        // hi*lo
+              wgmma_tf32<BN>(cor, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), 1u);       // lo*hi
+            }
+          }
+          wgmma_commit();
+          if (held >= 0) {                                   // one stage stays in flight: the previous one is complete now
+            wgmma_wait<1>();
+            release(held);
+          }
+          held = s;
+        }
+        wgmma_wait<0>();
+        release(held);
+        if constexpr (TERMS == 3) {
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) sum[j] += acc[j] + cor[j];   // fp32 RN adds
+        } else {
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) sum[j] += acc[j];
+        }
+      }
+      // ---- coalesced store in 16-column slabs: registers -> warp-private smem (transpose) -> 64-byte row segments
+#pragma unroll
+      for (int sl = 0; sl < BN / SLAB; ++sl) {
         __syncwarp();                                          // the previous slab has been read back by this warp
 #pragma unroll
-        for (int j = 0; j < SLAB; j += 4)
-          *reinterpret_cast<float4*>(&tile[lane * PITCH + j]) =
-              make_float4(sum[sl * SLAB + j], sum[sl * SLAB + j + 1], sum[sl * SLAB + j + 2], sum[sl * SLAB + j + 3]);
+        for (int jj = 0; jj < 2; ++jj) {                     // fragment column group j = 2 sl + jj: columns 8 jj + 2 (lane % 4) + {0, 1}
+          const int j = 2 * sl + jj, cc = 8 * jj + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(&tile[sub * PITCH + cc]) = make_float2(sum[4 * j], sum[4 * j + 1]);
+          *reinterpret_cast<float2*>(&tile[(sub + 8) * PITCH + cc]) = make_float2(sum[4 * j + 2], sum[4 * j + 3]);
+        }
         __syncwarp();
         const int col = n0 + sl * SLAB + cl;
-        if (col < d.Cout && !(p.dbg & 1)) {
-          float4 acc4[4], ra[4], rb[4];
-          int fl[4];
-          long long yo[4];
+        if (col < d.Cout) {
+          float4 acc4[2], ra[2], rb[2];
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {                       // batch the loads of 4 x 8 rows (memory-level parallelism)
-            const int lr = i * 8 + sub, rr = q * 32 + lr;
-            fl[i] = row_flag[rr];
-            yo[i] = row_y[rr];
-            acc4[i] = *reinterpret_cast<const float4*>(&tile[lr * PITCH + cl]);
+          for (int i = 0; i < 2; ++i) {                       // batch the loads of both rows (memory-level parallelism)
+            acc4[i] = *reinterpret_cast<const float4*>(&tile[(i * 8 + sub) * PITCH + cl]);
             ra[i] = make_float4(0.f, 0.f, 0.f, 0.f);
             rb[i] = ra[i];
             if (fl[i] & 1) {
-              if (p.res) ra[i] = *reinterpret_cast<const float4*>(p.res + row_r1[rr] + col);
-              if (p.res2) rb[i] = *reinterpret_cast<const float4*>(p.res2 + row_r2[rr] + col);
+              if (p.res) ra[i] = *reinterpret_cast<const float4*>(p.res + o1[i] + col);
+              if (p.res2) rb[i] = *reinterpret_cast<const float4*>(p.res2 + o2[i] + col);
             }
           }
 #pragma unroll
-          for (int i = 0; i < 4; ++i) {
+          for (int i = 0; i < 2; ++i) {
             if (!(fl[i] & 1)) continue;
             float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
             if (p.bias) bv = __ldg(reinterpret_cast<const float4*>(p.bias + (d.bias_n_mod ? (long long)((fl[i] >> 1) % d.bias_n_mod) * d.Cout : 0) + col));
             const float4 o = make_float4(acc4[i].x + bv.x + ra[i].x + rb[i].x, acc4[i].y + bv.y + ra[i].y + rb[i].y,
                                          acc4[i].z + bv.z + ra[i].z + rb[i].z, acc4[i].w + bv.w + ra[i].w + rb[i].w);
-            float* dst = p.y + ((p.dbg & 8) ? (long long)(threadIdx.x * 4) : yo[i] + col);   // dbg 8: all stores hit one hot 2 KB
+            float* dst = p.y + yo[i] + col;
             if (GATHER || p.splits > 1) {                      // taps / K splits race on an output row: red.add
               tt_red_add_v4(dst, o.x, o.y, o.z, o.w);
-            } else if (!(p.dbg & 16) || o.x == 12345.678f) {                                 // dbg 16: no store at all
+            } else {
               *reinterpret_cast<float4*>(dst) =
                   make_float4(tt_act(o.x, d.act), tt_act(o.y, d.act), tt_act(o.z, d.act), tt_act(o.w, d.act));
             }
           }
         }
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");         // everyone is done with the row tables before the next tile
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                       // no CTA leaves while its peer can still signal its barriers
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS));
   }
 }
 
@@ -518,6 +427,20 @@ __global__ void splitk_finish_kernel(const tt_conv_desc d, float* __restrict__ y
   }
 }
 
+// persistent grid: one CTA per SM (at most `max_ctas`) walks the `items` work items
+template <int TERMS, bool GATHER>
+cudaError_t launch_tc(const CUtensorMap& ma, const CUtensorMap& mb_hi, const CUtensorMap& mb_lo, const TcArgs& a, long long items,
+                      long long max_ctas, cudaStream_t st) {
+  // stage ring + 8 warp-private transposition slabs + barriers and the tap prefix
+  constexpr int smem = STAGES * (2 * BM * KS * 4 + 2 * BN * KS * 4) + 1024 + 8 * 16 * 20 * 4 + 512;
+  static_assert(smem <= 227 * 1024, "shared memory per block");
+  static bool set = false;
+  if (!set) { cudaFuncSetAttribute(conv_tc_kernel<TERMS, GATHER>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set = true; }
+  const long long grid = items < max_ctas ? items : max_ctas;
+  conv_tc_kernel<TERMS, GATHER><<<(unsigned)(grid > 1 ? grid : 1), NTHREADS, smem, st>>>(ma, mb_hi, mb_lo, a);
+  return cudaGetLastError();
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 }  // namespace
 
@@ -540,7 +463,7 @@ extern "C" size_t tt_conv2d_workspace_bytes(const tt_conv_desc* d) {
     const int s = tt_simt_splits(d, 0);
     return s > 1 ? (size_t)s * d->N * d->OH * d->OW * d->Cout * 4 : 0;
   }
-  return 0;                                                   // tcgen05: operands are split inside the kernel
+  return 0;                                                   // tensor cores: operands are split inside the kernel
 }
 
 // w_tc: [2][Cout][taps][Cin] fp32 = TF32-exact hi plane then lo plane (prepared once per layer by the host).
@@ -555,9 +478,7 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
   TcArgs a;
   a.d = *d;
   a.bias = bias; a.res = res; a.res2 = res2; a.y = y;
-  a.terms = terms;
-  a.chunk = terms == 3 ? ((g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2) : 16;   // 2 slabs = K 64: 8 truncating accumulations per chunk (4 slabs are 8% faster
-                                                              // end to end but fail the 1e-3 golden bound on one seed: tools/golden_err.py; debug bit 0x20000)
+  a.chunk = terms == 3 ? ((g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2) : 16;   // 2 slabs = K 64: 8 truncating accumulations per chunk
   a.n_slabs = (d->Cin + KS - 1) / KS;
   a.total_pix = d->N * d->OH * d->OW;
   a.flat = (taps == 1 && d->pad == 0 && d->stride == 1 && xhs == (long long)d->W * d->x_ld && xns == (long long)d->H * xhs) ? 1 : 0;
@@ -589,32 +510,28 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
     if (!encode_map(&ma, xa, 4, dims, str, box, d->stride)) return TT_ERR_CUDA;
     grid_x = a.tiles_w * a.tiles_h * d->N;
   }
-  // (a BN = 256 variant with merged accumulators was measured slower than BN = 128 with the fused hi*hi|hi*lo MMA: dropped)
-  const int BN = d->Cout > 64 ? 128 : 64;
   {
     const size_t wplane = (size_t)d->Cout * taps * d->Cin;
     cuuint64_t dims[3] = {(cuuint64_t)d->Cin, (cuuint64_t)taps, (cuuint64_t)d->Cout};
     cuuint64_t str[2] = {(cuuint64_t)d->Cin * 4, (cuuint64_t)taps * d->Cin * 4};
-    cuuint32_t box[3] = {KS, 1, (cuuint32_t)(BN / 2)};               // each CTA of a pair loads (and multicasts) half of the slab
+    cuuint32_t box[3] = {KS, 1, (cuuint32_t)(BN / 2)};               // a plane's BN-row slab is loaded as two half boxes
     if (!encode_map(&mb_hi, w_tc, 3, dims, str, box)) return TT_ERR_CUDA;
     if (!encode_map(&mb_lo, w_tc + wplane, 3, dims, str, box)) return TT_ERR_CUDA;
   }
-  a.dbg = g_tt_debug & 0xFF;
   a.m_tiles = grid_x;
   a.n_tiles = tt_cdiv(d->Cout, BN);
-  static int num_sms = 0;
-  if (!num_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev); }
+  const int num_sms = tt_num_sms();
   // split-K: a layer with few tiles and a long K (14x28 / 21x21 / 84x84 maps) leaves most SMs idle; spread K over
-  // the idle CTA pairs.  Needs a plain output layout (no pixel scatter, SAME residuals, one bias vector).
+  // the idle SMs.  Needs a plain output layout (no pixel scatter, SAME residuals, one bias vector).
   const int k_iters = taps * a.n_slabs;
   a.splits = 1;
   a.k_per = k_iters;
   {
-    const long long tile_pairs = (long long)((a.m_tiles + 1) / 2) * a.n_tiles;
+    const long long tiles = (long long)a.m_tiles * a.n_tiles;
     const bool plain = d->oy_mul == 1 && d->ox_mul == 1 && d->oy_add == 0 && d->ox_add == 0 && d->yH == d->OH && d->yW == d->OW &&
                        d->res_mode != TT_RES_UP2_NEAREST && d->bias_n_mod == 0 && !(g_tt_debug & 128);
-    if (plain && tile_pairs * 2 <= num_sms / 2 && k_iters >= 16) {
-      int sp = (int)((num_sms / 2 + tile_pairs - 1) / tile_pairs);
+    if (plain && tiles <= num_sms / 2 && k_iters >= 16) {
+      int sp = (int)((num_sms + tiles - 1) / tiles);
       if (sp > k_iters / 8) sp = k_iters / 8;
       if (sp > 32) sp = 32;
       if (sp >= 2) {
@@ -625,7 +542,7 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
   }
   if (a.splits > 1) {
     const long long total4 = (long long)d->N * d->OH * d->OW * (d->Cout / 4);
-    const int nb = (int)((total4 + 255) / 256 > 1184 ? 1184 : (total4 + 255) / 256);
+    const int nb = (int)((total4 + 255) / 256 > num_sms * 8 ? num_sms * 8 : (total4 + 255) / 256);
     splitk_init_kernel<<<nb, 256, 0, st>>>(*d, bias, d->res_mode != TT_RES_NONE ? res : nullptr, res2, y);
     ++g_tt_launches;
     TT_CHECK_LAUNCH("tt_conv2d(tc split-k init)");
@@ -633,45 +550,15 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
     a.d.act = TT_ACT_NONE;
     a.d.res_mode = TT_RES_NONE;
   }
-  const long long pairs = (long long)((a.m_tiles + 1) / 2) * a.n_tiles * a.splits;
-  const long long max_pairs = (num_sms - ((g_tt_debug >> 8) & 0xFF)) / 2;        // debug bits 8..15: SMs left to a concurrent branch
-  dim3 grid((unsigned)(2 * (pairs < max_pairs ? pairs : max_pairs)));  // persistent CTA pairs (cluster of 2), one CTA per SM
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  constexpr int EPI_BYTES = 8 * 32 * 20 * 4 + BM * (3 * 8 + 4) + 512;  // 8 warp-private slabs + row tables + barriers (13 x 8 B) + tap prefix
-  cudaError_t lerr;
-  if (BN == 128) {
-    constexpr int smem = 3 * (2 * BM * KS * 4 + 2 * 128 * KS * 4) + 1024 + EPI_BYTES;
-    static bool set128 = false;
-    if (!set128) { cudaFuncSetAttribute(conv_tc_kernel<128, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set128 = true; }
-    cfg.dynamicSmemBytes = smem;
-    lerr = cudaLaunchKernelEx(&cfg, conv_tc_kernel<128, 3, false>, ma, mb_hi, mb_lo, a);
-  } else if (g_tt_debug & 0x10000) {                          // experiment: 3-stage ring for BN = 64
-    constexpr int smem = 3 * (2 * BM * KS * 4 + 2 * 64 * KS * 4) + 1024 + EPI_BYTES;
-    static bool set64 = false;
-    if (!set64) { cudaFuncSetAttribute(conv_tc_kernel<64, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set64 = true; }
-    cfg.dynamicSmemBytes = smem;
-    lerr = cudaLaunchKernelEx(&cfg, conv_tc_kernel<64, 3, false>, ma, mb_hi, mb_lo, a);
-  } else {                                                    // BN = 64 stages are 48 KB: a 4-deep ring fits
-    constexpr int smem = 4 * (2 * BM * KS * 4 + 2 * 64 * KS * 4) + 1024 + EPI_BYTES;
-    static bool set64 = false;
-    if (!set64) { cudaFuncSetAttribute(conv_tc_kernel<64, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set64 = true; }
-    cfg.dynamicSmemBytes = smem;
-    lerr = cudaLaunchKernelEx(&cfg, conv_tc_kernel<64, 4, false>, ma, mb_hi, mb_lo, a);
-  }
-  if (lerr != cudaSuccess) { tt_set_error("tt_conv2d(tc): cluster launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
+  const long long items = (long long)a.m_tiles * a.n_tiles * a.splits;
+  const long long ctas = num_sms - ((g_tt_debug >> 8) & 0xFF);
+  const cudaError_t lerr = terms == 3 ? launch_tc<3, false>(ma, mb_hi, mb_lo, a, items, ctas, st) : launch_tc<1, false>(ma, mb_hi, mb_lo, a, items, ctas, st);   // debug bits 8..15: SMs left to a concurrent branch
+  if (lerr != cudaSuccess) { tt_set_error("tt_conv2d(tc): launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_conv2d(tc)");
   if (a.splits > 1 && d->act != TT_ACT_NONE) {
     const long long total4 = (long long)d->N * d->OH * d->OW * (d->Cout / 4);
-    const int nb = (int)((total4 + 255) / 256 > 1184 ? 1184 : (total4 + 255) / 256);
+    const int nb = (int)((total4 + 255) / 256 > num_sms * 8 ? num_sms * 8 : (total4 + 255) / 256);
     splitk_finish_kernel<<<nb, 256, 0, st>>>(*d, y);
     ++g_tt_launches;
     TT_CHECK_LAUNCH("tt_conv2d(tc split-k finish)");
@@ -698,15 +585,13 @@ int tt_sparse_conv_tc(const tt_sparse_conv_desc* d, const float* feats_in, const
   a.d.Cin = d->Cin; a.d.x_ld = d->in_ld; a.d.Cout = d->Cout; a.d.y_ld = d->out_ld;
   a.d.act = TT_ACT_NONE;
   a.y = feats_out;
-  a.terms = d->impl == 3 ? 3 : 1;
-  a.chunk = a.terms == 3 ? ((g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2) : 16;
+  const int terms = d->impl == 3 ? 3 : 1;
+  a.chunk = terms == 3 ? ((g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2) : 16;
   a.n_slabs = (d->Cin + KS - 1) / KS;
-  a.dbg = g_tt_debug & 0xFF;
   a.gx = feats_in; a.gx_ld = d->in_ld;
   a.pairs_in = pairs_in; a.pairs_out = pairs_out; a.pair_count = pair_count;
   a.kvol = d->kvol; a.pair_cap = d->pair_cap;
   a.splits = 1; a.k_per = a.n_slabs;
-  const int BN = d->Cout > 64 ? 128 : 64;
   a.n_tiles = tt_cdiv(d->Cout, BN);
   CUtensorMap mb_hi, mb_lo;
   {
@@ -717,35 +602,11 @@ int tt_sparse_conv_tc(const tt_sparse_conv_desc* d, const float* feats_in, const
     if (!encode_map(&mb_hi, w_tc, 3, dims, str, box)) return TT_ERR_CUDA;
     if (!encode_map(&mb_lo, w_tc + wplane, 3, dims, str, box)) return TT_ERR_CUDA;
   }
-  static int num_sms = 0;
-  if (!num_sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev); }
-  const long long cap_pairs = (long long)d->kvol * ((tt_cdiv(d->pair_cap, BM) + 1) / 2) * a.n_tiles;
-  const long long max_pairs = num_sms / 2;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * (cap_pairs < max_pairs ? cap_pairs : max_pairs)));
-  cfg.blockDim = dim3(NTHREADS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  constexpr int EPI_BYTES = 8 * 32 * 20 * 4 + BM * (3 * 8 + 4) + 512;
-  cudaError_t lerr;
-  if (BN == 128) {
-    constexpr int smem = 3 * (2 * BM * KS * 4 + 2 * 128 * KS * 4) + 1024 + EPI_BYTES;
-    static bool set128 = false;
-    if (!set128) { cudaFuncSetAttribute(conv_tc_kernel<128, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set128 = true; }
-    cfg.dynamicSmemBytes = smem;
-    lerr = cudaLaunchKernelEx(&cfg, conv_tc_kernel<128, 3, true>, mb_hi, mb_hi, mb_lo, a);
-  } else {
-    constexpr int smem = 3 * (2 * BM * KS * 4 + 2 * 64 * KS * 4) + 1024 + EPI_BYTES;
-    static bool set64 = false;
-    if (!set64) { cudaFuncSetAttribute(conv_tc_kernel<64, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set64 = true; }
-    cfg.dynamicSmemBytes = smem;
-    lerr = cudaLaunchKernelEx(&cfg, conv_tc_kernel<64, 3, true>, mb_hi, mb_hi, mb_lo, a);
-  }
-  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv(tc): cluster launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
+  const int num_sms = tt_num_sms();
+  const long long cap_items = (long long)d->kvol * tt_cdiv(d->pair_cap, BM) * a.n_tiles;   // upper bound of gathered tiles over all taps
+  const cudaError_t lerr = terms == 3 ? launch_tc<3, true>(mb_hi, mb_hi, mb_lo, a, cap_items, num_sms, st)
+                                        : launch_tc<1, true>(mb_hi, mb_hi, mb_lo, a, cap_items, num_sms, st);
+  if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv(tc): launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv(tc)");
   return TT_OK;

@@ -250,7 +250,7 @@ int tt_voxel_pooling_forward(int batch_size, int num_points, int num_channels, i
                    ((reinterpret_cast<uintptr_t>(output_features) & 15) == 0);
   const int CV = vec ? num_channels / 4 : num_channels;
   const long long total = tp * CV;
-  const int blocks = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int blocks = (int)((total + 255) / 256 > tt_num_sms() * 32 ? tt_num_sms() * 32 : (total + 255) / 256);
   if (vec)
     voxel_pool_kernel<true><<<blocks, 256, 0, st>>>(total, num_points, num_channels, CV, num_voxel_x, num_voxel_y,
                                                      num_voxel_z, geom_xyz, input_features, output_features);

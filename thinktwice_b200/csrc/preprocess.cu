@@ -171,7 +171,7 @@ int tt_preprocess_u8(const tt_preproc_desc* d, const uint8_t* raw, const float* 
   const long long total = (long long)d->n_img * d->outH * d->outW;
   if (total == 0) return TT_OK;
   const long long want = (total + 255) / 256;
-  const int nb = (int)(want > 148 * 16 ? 148 * 16 : want);
+  const int nb = (int)(want > tt_num_sms() * 16 ? tt_num_sms() * 16 : want);
   preprocess_u8_kernel<<<nb, 256, 0, (cudaStream_t)stream>>>(raw, reinterpret_cast<const float2*>(map_grid), out_nchw, static_cast<__half*>(out_split8),
                                                              split_plane, *d, total);
   ++g_tt_launches;

@@ -1,4 +1,4 @@
-"""EncoderDecoder — the model entry point, B200-native.
+"""EncoderDecoder — the model entry point, H100-native.
 
 Drop-in for the reference class of the same name (open_loop_training/code/encoder_decoder_framework.py):
 same registry name, same constructor keywords, same `forward_inference(batch)` / `process_action` /
@@ -95,7 +95,7 @@ class EncoderDecoder(nn.Module):
         dev = torch.device(device)
         lib.require_cuda(dev)
         if impl == lib.IMPL_AUTO:
-            impl = lib.IMPL_F16S                                    # default engine: tcgen05 on scaled-split fp16 operands (fp32-class)
+            impl = lib.IMPL_F16S                                    # default engine: tensor cores on scaled-split fp16 operands (fp32-class)
         self.eng = e = Engine(dev, impl)
         pk = Packer(self.state_dict(), dev, tc_mode=impl if impl in (lib.IMPL_TF32, lib.IMPL_3XTF32, lib.IMPL_F16S) else 0)
         self.img_encoder.prepare(pk, e)

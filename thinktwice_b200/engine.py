@@ -72,8 +72,8 @@ class PackedConv:
 
     def __init__(self, w, bias, Cin, Cout, KH=1, KW=1, groups=1, w_tc=None, w_h=None):
         self.w, self.bias, self.Cin, self.Cout, self.KH, self.KW, self.groups = w, bias, Cin, Cout, KH, KW, groups
-        self.w_tc = w_tc            # [2][Cout][taps][Cin] TF32 hi / lo planes for the tcgen05 3xTF32 path (or None)
-        self.w_h = w_h              # [2][Cout][taps][Cin8] scaled-split fp16 planes for the tcgen05 f16s path (or None)
+        self.w_tc = w_tc            # [2][Cout][taps][Cin] TF32 hi / lo planes for the tensor-core 3xTF32 path (or None)
+        self.w_h = w_h              # [2][Cout][taps][Cin8] scaled-split fp16 planes for the tensor-core f16s path (or None)
         self.alg_k = None           # algorithmic K per output (row-packed convs carry zero-weight padding)
 
 
@@ -309,7 +309,7 @@ class Engine:
         if res2 is not None:
             d.res2_ld, d.res2_coff = res2.ld, 0
         impl = self.impl if impl is None else impl
-        # tcgen05 paths: dense convs with enough work to fill 128-row tiles; everything else stays SIMT fp32
+        # tensor-core paths: dense convs with enough work to fill 128-row tiles; everything else stays SIMT fp32
         big = (d.N * OH * OW >= self.tc_min_rows or (d.N * OH * OW >= 128 and pw.KH * pw.KW * pw.Cin >= 2048))   # thin M: only with a long K (split-K)
         common = (stride in self.tc_strides and pw.groups == 1 and out.ld % 4 == 0 and out.coff % 4 == 0
                   and (res is None or (res.ld % 4 == 0 and res.coff % 4 == 0)) and (res2 is None or (res2.ld % 4 == 0 and res2.coff % 4 == 0))
@@ -329,7 +329,7 @@ class Engine:
             self._cur_name = name
             xs = self.with_split(x)
         ws = None
-        need = 0 if use_h else lib.load().tt_conv2d_workspace_bytes(C.byref(d))    # SIMT: split-K partials; tcgen05: 0
+        need = 0 if use_h else lib.load().tt_conv2d_workspace_bytes(C.byref(d))    # SIMT: split-K partials; tensor cores: 0
         if need:
             ws = self.conv_ws.get(self.lane)
             if ws is None or ws.numel() < need:

@@ -89,7 +89,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise TTError(f'{LIB_PATH} is missing: run `python -c "import __graft_entry__ as g; g.build()"` '
-                      '(nvcc, sm_100a).  thinktwice_b200 has no CPU / eager fallback.')
+                      '(nvcc, sm_90a).  thinktwice_b200 has no CPU / eager fallback.')
     lib = C.CDLL(LIB_PATH)
     lib.tt_last_error.restype = C.c_char_p
     lib.tt_launch_count.restype = C.c_longlong
@@ -97,7 +97,7 @@ def load():
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
-        lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0))
+        check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
     _lib = lib
     return lib
 

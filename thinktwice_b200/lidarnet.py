@@ -1,4 +1,4 @@
-"""LiDAR -> BEV encoder on the B200 op library.
+"""LiDAR -> BEV encoder on the H100 op library.
 
 Mirror of the reference `LidarNet` / `SparseEncoder_fp32` (open_loop_training/code/model_code/backbones/
 lidarnet.py:24-96, cfg configs/thinktwice.py:159-193): hard voxelisation + mean VFE, the sparse 3-D

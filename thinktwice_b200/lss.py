@@ -1,4 +1,4 @@
-"""Camera -> BEV encoder on the B200 op library.
+"""Camera -> BEV encoder on the H100 op library.
 
 Mirror of the reference `LSS` backbone (open_loop_training/code/model_code/backbones/lss.py:351-724):
 same constructor arguments, same forward(img, img_metas) contract, same output dict keys.  All tensor
@@ -85,7 +85,7 @@ class LSS(nn.Module):
         w['aspp'] = [pk.conv(f'{a}aspp{i + 1}.atrous_conv', bn=f'{a}aspp{i + 1}.bn') for i in range(4)]
         w['aspp_gap'] = pk.conv(a + 'global_avg_pool.1', bn=a + 'global_avg_pool.2')
         w['aspp_out'] = pk.conv(a + 'conv1', bn=a + 'bn1')
-        w['dcn_off'] = pk.conv(d + 'depth_conv.4.conv_offset', cout_pad=32)   # 18 -> 32 channels: tcgen05 instead of SIMT
+        w['dcn_off'] = pk.conv(d + 'depth_conv.4.conv_offset', cout_pad=32)   # 18 -> 32 channels: tensor cores instead of SIMT
         w['dcn'] = pk.conv_group_gemms(d + 'depth_conv.4', groups=4)   # one GEMM per group over the sampled columns
         w['depth_out'] = pk.conv(d + 'depth_conv.5')
         u = p + 'seg_net.'
@@ -93,7 +93,7 @@ class LSS(nn.Module):
             w[f'u{l}_up'] = pk.convT(f'{u}unet_layer{l}.up')
             w[f'u{l}_conv'] = pk.conv(f'{u}unet_layer{l}.conv_relu.0')
         w['u0_a'] = pk.conv(u + 'unet_layer0.1'); w['u0_b'] = pk.conv(u + 'unet_layer0.3')
-        w['seg_last'] = pk.conv(u + 'conv_last', cout_pad=32)          # 12 -> 32 zero-padded channels: tcgen05 instead of SIMT
+        w['seg_last'] = pk.conv(u + 'conv_last', cout_pad=32)          # 12 -> 32 zero-padded channels: tensor cores instead of SIMT
         self.seg_classes = int(pk.sd[u + 'conv_last.weight'].shape[0])
         r = p + 'seg_res_to_image_feature.'
         w['s2f'] = [pk.conv(f'{r}{3 * i}', bn=f'{r}{3 * i + 1}', cout_pad=32) for i in range(7)]   # s2f.1 is 64 -> 16

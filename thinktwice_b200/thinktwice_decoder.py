@@ -1,4 +1,4 @@
-"""ThinkTwiceDecoder — coarse heads + K x (Prediction, Look, Refine) on the B200 op library.
+"""ThinkTwiceDecoder — coarse heads + K x (Prediction, Look, Refine) on the H100 op library.
 
 Mirror of open_loop_training/code/model_code/dense_heads/thinktwice_decoder.py:262-489 (forward only),
 with the Look module's SpatialCrossAttention / MSDeformableAttention3D
@@ -204,7 +204,10 @@ class ThinkTwiceDecoder(nn.Module):
                 e.conv(meta['fpn'][l], L['value'][l], out=out, name=f'look.value{l}', y_nstride=nk * 256, bias_n_mod=cams)
         off = e.linear(q, L['off'], name='look.off')
         aw = e.linear(q, L['aw'], name='look.aw')
-        att = e.fmap('look.att', B * cams * cap, 1, 1, 256)
+        # tt_msda_forward writes the first max_len rows of each (frame, camera) only; the FFN below runs over all `cap` rows (static
+        # shapes for graph replay) and tt_look_reduce reads the valid ones.  Zero-filled once, so that the rows no forward has written yet
+        # hold zeros instead of stale memory, which look.ffn2's epilogue would split into fp16 planes and count as saturated
+        att = e.fmap('look.att', B * cams * cap, 1, 1, 256, zero=True)
         md = meta['msda_desc']
         md.value_ld, md.value_coff = (self.K * 256, k * 256) if meta['value_all'] is not None else (0, 0)
         lib.call('tt_msda_forward', C.byref(md), _p(value), _p(off.t), _p(aw.t), _p(ref_re), _p(max_len), _p(att.t))

@@ -23,7 +23,7 @@ def _rn_tf32(w):
 
 def tf32_split(w, rn=True):
     """w (fp32) -> (hi, lo) with hi = RN_tf32(w), lo = RN_tf32(w - hi): both exactly TF32-representable — the same
-    split the tcgen05 kernel applies to the activations in shared memory (csrc/gemm_conv_tc.cu: split_rn)."""
+    split the tensor-core kernel applies to the activations in shared memory (csrc/gemm_conv_tc.cu: split_rn)."""
     w = w.float().contiguous()
     hi = _rn_tf32(w)
     return hi, _rn_tf32(w - hi)

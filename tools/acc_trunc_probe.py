@@ -1,9 +1,9 @@
-"""Probe how the tcgen05 fp32 accumulator rounds (round 2 experiment, ~10 s of GPU time).
+"""Probe how the tensor-core fp32 accumulator rounds (round 2 experiment, ~10 s of GPU time).
 
 DESIGN.md §2: the dominant error of the 3xTF32 path is the truncating accumulate inside the tensor core.  If the
 truncation is toward zero, draining `acc + n_acc * 0.5 ulp(acc) * sign(acc)` would centre the error and allow
 4-8 K-slab chunks (8 % faster) at the accuracy of 2-slab chunks.  This script measures the SIGNED error of a single-pass
-TF32 1x1 convolution (impl 2: hi*hi only, one TMEM chunk of up to 16 K-slabs) whose operands are exactly
+TF32 1x1 convolution (impl 2: hi*hi only, one accumulator chunk of up to 16 K-slabs) whose operands are exactly
 TF32-representable, so every product is exact and the only rounding is the accumulate:
 
   * all-positive products  -> mean error / ulp(result)

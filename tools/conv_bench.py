@@ -54,7 +54,7 @@ def main():
                 x.t.copy_(xt)
                 eng.sync_split(x)
             for dbg in (dbg_list if impl > 1 else [0]):
-                L.tt_debug_set(dbg)
+                lib.check(L.tt_debug_set(dbg), 'tt_debug_set')
                 us = run(eng, x, pw, res, k, stride, pad)
                 line += f' | {tag}{"/d%d" % dbg if dbg else ""} {us:7.1f}us {gf / us * 1e3:6.1f}TF/s'
             L.tt_debug_set(0)

@@ -24,8 +24,7 @@ def rel(a, b):
 
 def main():
     cfg = Config.fromfile(PLUMBING_CONFIG)
-    variants = [('simt fp32', 1, 0), ('3xtf32', 3, 0), ('3xtf32 chunk2', 3, 0x20000), ('3xtf32 rn-lo', 3, 64),
-                ('3xtf32 chunk2+rn-lo', 3, 0x20000 | 64), ('3xtf32 no-splitk', 3, 128)]
+    variants = [('simt fp32', 1, 0), ('3xtf32', 3, 0), ('3xtf32 chunk4', 3, 0x20000), ('3xtf32 no-splitk', 3, 128)]
     for seed in (0, 1, 2):
         o = Oracle(**{k: v for k, v in cfg.model.items() if k != 'type'})
         init_oracle_weights(o, seed)
@@ -33,7 +32,7 @@ def main():
         calibrate_bn(o, batch)
         ref = np.load(os.path.join(G, f'plumbing_seed{seed}.npz'))
         for name, impl, dbg in variants:
-            lib.load().tt_debug_set(dbg)
+            lib.check(lib.load().tt_debug_set(dbg), 'tt_debug_set')
             m = build_model(cfg.model)
             m.load_state_dict(o.state_dict())
             m.prepare('cuda:0', impl=impl)

@@ -1,7 +1,7 @@
-"""BASELINE.json configs[4]: decoder-depth sweep K in {1, 2, 3, 5, 10} at a fixed encoder, one B200 — frames/s at the throughput
-batch (32 frames per forward) and per-frame latency at B = 1, device-timed CUDA-graph replays with resident inputs.
+"""BASELINE.json configs[4]: decoder-depth sweep K in {1, 2, 3, 5, 10} at a fixed encoder, one H100 — frames/s at the throughput
+batch (16 frames per forward: 32 do not fit 80 GB) and per-frame latency at B = 1, device-timed CUDA-graph replays with resident inputs.
 
-  python tools/k_sweep.py [--batch 32] [--ks 1,2,3,5,10] > gpurun_out/r2_k_sweep.json
+  python tools/k_sweep.py [--batch 16] [--ks 1,2,3,5,10] > k_sweep.json
 
 Weights: the bench's synthetic calibrated checkpoint (K = 5); decoder layers beyond the fifth keep the model's seeded init, layers
 the checkpoint has but the model lacks are dropped — the encoder is identical in every run.  Parity per K is the test suite's job
@@ -50,7 +50,7 @@ def measure(cfg, sd, K, B, steps, dev):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument('--batch', type=int, default=32)
+    ap.add_argument('--batch', type=int, default=16)
     ap.add_argument('--ks', default='1,2,3,5,10')
     args = ap.parse_args()
     from bench import synthetic_checkpoint
@@ -62,7 +62,7 @@ def main():
         for B, steps in ((args.batch, 3), (1, 20)):
             try:
                 rows.append(measure(Config.fromfile(DEFAULT_CONFIG), sd, K, B, steps, dev))
-            except torch.OutOfMemoryError as ex:                      # K = 10 at B = 32 may not fit beside the arena: say so, keep going
+            except torch.OutOfMemoryError as ex:                      # K = 10 at B = 16 may not fit beside the arena: say so, keep going
                 torch.cuda.empty_cache()
                 rows.append({'K': K, 'batch': B, 'error': repr(ex)[:200]})
             print(rows[-1], file=sys.stderr, flush=True)
@@ -70,7 +70,7 @@ def main():
     for r in rows:
         if 'ms_per_step' in r and r['batch'] in base:
             r['ms_over_K1'] = r['ms_per_step'] - base[r['batch']]['ms_per_step']
-    print(json.dumps({'workload': 'configs[4]: decoder-depth sweep at fixed encoder, thinktwice.py shape, 1 x B200, CUDA-graph replay, inputs resident',
+    print(json.dumps({'workload': 'configs[4]: decoder-depth sweep at fixed encoder, thinktwice.py shape, 1 x H100, CUDA-graph replay, inputs resident',
                       'rows': rows}))
 
 

@@ -8,7 +8,7 @@ capture"), in a single application run:
 The forward launches ~700 kernels; profiling all of them with ~40 replays each would take the whole GPU budget.  This driver
 runs warm-up steps unprofiled, then one eager step in which cudaProfilerStart/Stop brackets only the FIRST occurrence(s) of
 each C-ABI op (and of a chosen list of dominant conv layers), so the report holds a few launches of every kernel.
-tools/ncu_summary.py turns the report into profiles/*.md / *.json.
+tools/ncu_summary.py turns the report into *.md / *.json.
 """
 import argparse
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Top stall locations of one profiled kernel (needs a report captured with --import-source on; runs HERE, no GPU):
-   python tools/ncu_source_top.py gpurun_out/r2_f16s_3x3.ncu-rep profiles/r2_f16s_3x3_source.md "title"
+   python tools/ncu_source_top.py r2_f16s_3x3.ncu-rep f16s_3x3_source.md "title"
 """
 import csv
 import io

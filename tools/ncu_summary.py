@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an `ncu --set full` report into per-kernel roofline rows (run HERE, no GPU needed):
 
-  python tools/ncu_summary.py gpurun_out/r2_ops.ncu-rep profiles/r2_kernels [--peaks MEASURED_PEAKS.json]
+  python tools/ncu_summary.py r2_ops.ncu-rep r2_kernels [--peaks MEASURED_PEAKS.json]
 
 writes <out>.json (one record per profiled launch) and <out>.md (one table row per launch): duration, DRAM bytes read + written,
 achieved DRAM GB/s against the measured copy bandwidth, tensor-pipe active %, L2 -> SM bytes, shared-memory bank-conflict share.

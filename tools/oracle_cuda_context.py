@@ -1,5 +1,5 @@
 """Context number for the record (VERDICT r1 item 10; NOT a bench arm and not a parity check): the plain-PyTorch oracle of the same
-forward run on torch-CUDA (cuDNN / cuBLAS) on the same B200, with TF32 off (strict fp32 — the arithmetic class of this repo's f16s
+forward run on torch-CUDA (cuDNN / cuBLAS) on the same GPU, with TF32 off (strict fp32 — the arithmetic class of this repo's f16s
 engine) and TF32 on (what the reference executes on Ampere+ by default for convolutions).  B = 1, thinktwice.py config.
 
   python tools/oracle_cuda_context.py > gpurun_out/r2_oracle_cuda.json
