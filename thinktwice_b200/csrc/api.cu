@@ -28,7 +28,7 @@ const char* tt_last_error(void) { return g_err; }
 long long tt_launch_count(void) { return g_tt_launches; }
 int tt_debug_set(int flags) {
   // the knobs the kernels read (include/tt_b200.h); anything else is refused so that no experiment silently measures the default path
-  const int known = 128 | 0xFF00 | 0x20000 | 0x40000 | 0x200000;
+  const int known = 128 | 0xFF00 | 0x20000 | 0x40000 | 0x200000 | 0x400000;
   if (flags & ~known) {
     tt_set_error("tt_debug_set: unknown knob bits 0x%x", flags & ~known);
     return TT_ERR_INVALID;

@@ -18,7 +18,8 @@
 // Tiling follows gemm_conv_tc.cu: TMA box loads per tap (zero fill = padding, element strides = stride 2), persistent CTAs
 // (one per SM), split-K and GATHER (sparse convolution).
 // Warp roles: warpgroup 0 = producer (warp 0: TMA / gather; warps 1..3 idle);
-// warpgroups 1 and 2 = wgmma + epilogue for rows 0..63 / 64..127 of the tile.
+// warpgroups 1 and 2 = wgmma + epilogue for rows 0..63 / 64..127 of the tile.  The producer keeps 40 registers per thread (88 when
+// it gathers) and the MMA warpgroups take the rest (setmaxnreg), which lets a 128-column tile keep its 192 accumulators in registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -36,6 +37,12 @@ namespace {
 constexpr int BM = 128;           // M tile: two warpgroups x 64 rows
 constexpr int KE = 64;            // K elements per stage (one 128-byte swizzle row of halves)
 constexpr int NTHREADS = 384;     // warpgroup 0 producer, warpgroups 1..2 MMA + epilogue
+// registers per thread after setmaxnreg (a 384-thread CTA starts with 168): the TMA producer is one thread with a handful of
+// values; the gather producer (sparse modes) keeps row indices of several stages in flight and needs more
+template <bool GATHER> constexpr int reg_producer() { return GATHER ? 88 : 40; }
+template <bool GATHER> constexpr int reg_mma() { return GATHER ? 208 : 232; }
+static_assert(128 * reg_producer<false>() + 256 * reg_mma<false>() <= 168 * NTHREADS &&
+              128 * reg_producer<true>() + 256 * reg_mma<true>() <= 168 * NTHREADS, "setmaxnreg must not ask for more than the CTA holds");
 constexpr float LO_SCALE = 2048.f, LO_INV = 1.f / 2048.f;
 constexpr int MAX_KVOL = 32;
 constexpr float H_MAX = 65504.f;
@@ -185,6 +192,7 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   };
 
   if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(reg_producer<GATHER>()));
     if (warp == 0 && GATHER) {
       // ===================================================================== gather producer (whole warp) + weight TMA
       const uint32_t txb = 2 * B_BYTES;
@@ -329,6 +337,7 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
   } else {
     // ===================================================================== MMA + epilogue (warpgroups 1, 2)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(reg_mma<GATHER>()));
     const int cw = warp - 4;                                // MMA warp 0..7
     const int wg = cw >> 2;                                 // warpgroup: tile rows [64 wg, 64 wg + 64)
     const int row0 = wg * 64 + (cw & 3) * 16;               // this warp's 16 accumulator rows
@@ -342,9 +351,53 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       int nt, mt, tap, count, kb, ke;
       decode(pt, nt, mt, tap, count, kb, ke);
       const int nch = (ke - kb + p.chunk - 1) / p.chunk;
+      // ---- K walk: chunks of `chunk` stages accumulated by the tensor core, folded into fp32 sums with RN FMAs
+      float sum[BN / 2];
+#pragma unroll
+      for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
+      auto release = [&](int s) {                            // this warp's wgmmas no longer read stage s
+        __syncwarp();
+        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
+      };
+      int it = kb;
+      for (int c = 0; c < nch; ++c) {
+        // main and correction accumulators.  The first wgmma of a chunk overwrites them (scale-d 0), but the asm operands are
+        // read-write: without a definition here they would count as live around the work-item loop, through the epilogue.
+        float acc[BN / 2], cor[BN / 2];
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[j] = cor[j] = 0.f;
+        const int it_end = min(it + p.chunk, ke);
+        int held = -1;                                       // the stage whose wgmmas may still be in flight
+        for (bool first = true; it < it_end; ++it, ++ig, first = false) {
+          const int s = ig % STAGES;
+          mbar_wait(&full[s], (ig / STAGES) & 1);
+          if (GATHER) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async rows -> visible to wgmma
+          const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES) + wg * (A_BYTES / 2), a_lo = a_hi + A_BYTES;
+          const uint32_t b_hi = smem_u32(smem + s * STAGE_BYTES) + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < KE / 16; ++kk) {             // K = 16 halves = 32 bytes inside the 128-byte swizzle row
+            const uint32_t off = kk * 32, z = (first && kk == 0) ? 0u : 1u;
+            wgmma_f16<BN>(acc, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), z);    // hi*hi
+            wgmma_f16<BN>(cor, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), z);    // hi*lo'
+            wgmma_f16<BN>(cor, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), 1u);   // lo'*hi
+          }
+          wgmma_commit();
+          if (held >= 0) {                                   // one stage stays in flight: the previous one is complete now
+            wgmma_wait<1>();
+            release(held);
+          }
+          held = s;
+        }
+        wgmma_wait<0>();
+        release(held);
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) sum[j] += fmaf(cor[j], LO_INV, acc[j]);
+      }
+      // ---- output / residual addresses of the two rows this lane stores (rows row0 + sub, row0 + 8 + sub); computed after the
+      // K walk so that they do not hold registers across it
       const bool real_tile = GATHER ? mt * BM < count : mt < p.m_tiles;
       const int n0 = nt * BN;
-      // ---- output / residual addresses of the two rows this lane stores (rows row0 + sub, row0 + 8 + sub)
       int fl[2];
       long long yo[2], o1[2], o2[2];
 #pragma unroll
@@ -388,45 +441,6 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           yo[i] = nimg * yns + ((long long)(oh * d.oy_mul + d.oy_add) * d.yW + ow * d.ox_mul + d.ox_add) * d.y_ld + d.y_coff;
           fl[i] = (valid ? 1 : 0) | (nimg << 1);
         }
-      }
-      // ---- K walk: chunks of `chunk` stages accumulated by the tensor core, folded into fp32 sums with RN FMAs
-      float sum[BN / 2];
-#pragma unroll
-      for (int j = 0; j < BN / 2; ++j) sum[j] = 0.f;
-      auto release = [&](int s) {                            // this warp's wgmmas no longer read stage s
-        __syncwarp();
-        if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&empty[s])) : "memory");
-      };
-      int it = kb;
-      for (int c = 0; c < nch; ++c) {
-        float acc[BN / 2], cor[BN / 2];                      // main and correction accumulators
-        const int it_end = min(it + p.chunk, ke);
-        int held = -1;                                       // the stage whose wgmmas may still be in flight
-        for (bool first = true; it < it_end; ++it, ++ig, first = false) {
-          const int s = ig % STAGES;
-          mbar_wait(&full[s], (ig / STAGES) & 1);
-          if (GATHER) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // cp.async rows -> visible to wgmma
-          const uint32_t a_hi = smem_u32(smem + s * STAGE_BYTES) + wg * (A_BYTES / 2), a_lo = a_hi + A_BYTES;
-          const uint32_t b_hi = smem_u32(smem + s * STAGE_BYTES) + 2 * A_BYTES, b_lo = b_hi + B_BYTES;
-          wgmma_fence();
-#pragma unroll
-          for (int kk = 0; kk < KE / 16; ++kk) {             // K = 16 halves = 32 bytes inside the 128-byte swizzle row
-            const uint32_t off = kk * 32, z = (first && kk == 0) ? 0u : 1u;
-            wgmma_f16<BN>(acc, make_smem_desc(a_hi + off), make_smem_desc(b_hi + off), z);    // hi*hi
-            wgmma_f16<BN>(cor, make_smem_desc(a_hi + off), make_smem_desc(b_lo + off), z);    // hi*lo'
-            wgmma_f16<BN>(cor, make_smem_desc(a_lo + off), make_smem_desc(b_hi + off), 1u);   // lo'*hi
-          }
-          wgmma_commit();
-          if (held >= 0) {                                   // one stage stays in flight: the previous one is complete now
-            wgmma_wait<1>();
-            release(held);
-          }
-          held = s;
-        }
-        wgmma_wait<0>();
-        release(held);
-#pragma unroll
-        for (int j = 0; j < BN / 2; ++j) sum[j] += fmaf(cor[j], LO_INV, acc[j]);
       }
       // ---- coalesced store in 16-column slabs: registers -> warp-private smem (transpose) -> 64-byte row segments
 #pragma unroll
@@ -738,13 +752,15 @@ __global__ void f16s_sparse_init_kernel(float* __restrict__ y, int y_ld, const f
 
 // shared memory beyond the stage ring: 8 warp-private transposition slabs, barriers and the tap prefix
 constexpr int EPI_BYTES = 8 * 16 * 20 * 4 + 512;
-// N tile: each MMA thread holds BN fp32 accumulators (BN / 2 main + BN / 2 corr) plus BN / 2 fp32 sums; at 384 threads
-// per CTA the compiler's budget is 168 registers per thread, which BN = 128 (192 live accumulators) overflows
-constexpr int BN = 64, STAGES = 4;
+// N tiles: each MMA thread holds BN / 2 main + BN / 2 correction accumulators plus BN / 2 fp32 sums, 96 registers at BN = 64 and
+// 192 at BN = 128 (within the 232 setmaxnreg gives the MMA warpgroups).  A BN = 128 stage is 64 KB, so its ring is 3 stages deep;
+// BN = 64 keeps 4 stages of 48 KB.  The sparse modes (GM 1 / 2) always use BN = 64.
+constexpr int BN_NARROW = 64, BN_WIDE = 128;
 
 // persistent grid: one CTA per SM walks the (M unit, N tile, K split) work items; debug bits 8..15: SMs left to a concurrent branch
-template <int GM>
+template <int BN, int GM>
 cudaError_t launch_f16s(const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a, long long m_units, cudaStream_t st) {
+  constexpr int STAGES = BN == BN_WIDE ? 3 : 4;
   constexpr int smem = STAGES * (2 * BM * KE * 2 + 2 * BN * KE * 2) + 1024 + EPI_BYTES;
   static_assert(smem <= 227 * 1024, "shared memory per block");
   static bool set = false;
@@ -944,10 +960,18 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
     if (!encode_map(&ma, x_split, 5, dims, str, box, d->stride, CU_TENSOR_MAP_DATA_TYPE_FLOAT16)) return TT_ERR_CUDA;
     grid_x = a.tiles_w * a.tiles_h * d->N;
   }
-  if (!encode_weights(&mb, w_split, d->Cin, taps, d->Cout, BN)) return TT_ERR_CUDA;
   a.m_tiles = grid_x;
-  a.n_tiles = tt_cdiv(d->Cout, BN);
   const int num_sms = tt_num_sms();
+  // 128-column tiles read each A slab once per 128 output channels instead of 64 and need less shared-memory bandwidth per MMA.
+  // They are used when Cout > 64 and the 128-column tiles alone give every SM one, so they never run split-K.  tools/conv_bench.py
+  // on an H100 SXM: with N = 64 every shape with Cout >= 128 was 3-17 % faster on 128-column tiles (400 W card), while N = 4 layer4
+  // convs that needed split-K to fill the SMs with 128-column tiles were 1.5-1.6x slower (700 W card: 77 vs 51 us for 3x3
+  // 512 -> 512 at 14 x 28, 49 vs 31 us for 1x1 2048 -> 512).
+  // Debug bit 0x400000 forces BN = 64 (A/B of the two tiles in one build).
+  const bool wide = d->Cout > BN_NARROW && !(g_tt_debug & 0x400000) && (long long)a.m_tiles * tt_cdiv(d->Cout, BN_WIDE) >= num_sms;
+  const int bn = wide ? BN_WIDE : BN_NARROW;
+  if (!encode_weights(&mb, w_split, d->Cin, taps, d->Cout, bn)) return TT_ERR_CUDA;
+  a.n_tiles = tt_cdiv(d->Cout, bn);
   const int k_iters = taps * a.n_slabs;
   a.splits = 1;
   a.k_per = k_iters;
@@ -976,7 +1000,7 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
     a.d.act = TT_ACT_NONE;
     a.d.res_mode = TT_RES_NONE;
   }
-  const cudaError_t lerr = launch_f16s<0>(ma, mb, a, a.m_tiles, st);
+  const cudaError_t lerr = bn == BN_WIDE ? launch_f16s<BN_WIDE, 0>(ma, mb, a, a.m_tiles, st) : launch_f16s<BN_NARROW, 0>(ma, mb, a, a.m_tiles, st);
   if (lerr != cudaSuccess) { tt_set_error("tt_conv2d_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_conv2d_f16s");
@@ -1020,11 +1044,11 @@ int tt_sparse_conv_f16s(const tt_sparse_conv_desc* d, const void* feats_in_split
   a.pairs_in = pairs_in; a.pairs_out = pairs_out; a.pair_count = pair_count;
   a.kvol = d->kvol; a.pair_cap = d->pair_cap;
   a.splits = 1; a.k_per = a.n_slabs;
-  a.n_tiles = tt_cdiv(d->Cout, BN);
+  a.n_tiles = tt_cdiv(d->Cout, BN_NARROW);
   CUtensorMap mb;
-  if (!encode_weights(&mb, w_split, d->Cin, d->kvol, d->Cout, BN)) return TT_ERR_CUDA;
+  if (!encode_weights(&mb, w_split, d->Cin, d->kvol, d->Cout, BN_NARROW)) return TT_ERR_CUDA;
   const long long cap_units = (long long)d->kvol * tt_cdiv(d->pair_cap, BM);      // upper bound of gathered M tiles over all taps
-  const cudaError_t lerr = launch_f16s<1>(mb, mb, a, cap_units, st);
+  const cudaError_t lerr = launch_f16s<BN_NARROW, 1>(mb, mb, a, cap_units, st);
   if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_f16s");
@@ -1065,11 +1089,11 @@ int tt_sparse_conv_os_f16s(const tt_sparse_conv_desc* d, const tt_f16s_io* io, c
   a.kvol = d->kvol; a.nbr = nbr; a.out_count = out_count; a.cap_rows = d->cap_out;
   a.tps = (d->Cin == 32 && !(g_tt_debug & 0x200000)) ? 2 : 1;
   a.splits = 1; a.k_per = a.tps == 2 ? (d->kvol + 1) / 2 : d->kvol * a.n_slabs;
-  a.n_tiles = tt_cdiv(d->Cout, BN);
+  a.n_tiles = tt_cdiv(d->Cout, BN_NARROW);
   CUtensorMap mb;
-  if (!encode_weights(&mb, io->w_split, d->Cin, d->kvol, d->Cout, BN, a.tps == 2)) return TT_ERR_CUDA;
+  if (!encode_weights(&mb, io->w_split, d->Cin, d->kvol, d->Cout, BN_NARROW, a.tps == 2)) return TT_ERR_CUDA;
   const long long cap_units = tt_cdiv(d->cap_out, BM);
-  const cudaError_t lerr = launch_f16s<2>(mb, mb, a, cap_units, (cudaStream_t)stream);
+  const cudaError_t lerr = launch_f16s<BN_NARROW, 2>(mb, mb, a, cap_units, (cudaStream_t)stream);
   if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_os_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_os_f16s");
