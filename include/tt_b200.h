@@ -329,6 +329,18 @@ int tt_msda_forward(const tt_msda_desc* d, const float* value, const float* off,
 /* msda:338-342: zero the first B rows of every (b, cam), divide by B, sum rows < max_len -> [B][cams*C] */
 int tt_look_reduce(const float* rows, int B, int cams, int cap, int C, const int* max_len, float* out,
                    tt_stream_t stream);
+/* Independent frames: every frame of the batch computed as the reference computes it alone, at B = 1 (the closed-loop agent's
+ * batch, leaderboard/team_code/thinktwice_agent.py:446-454).  The reference's row bound is the max_len of thinktwice_decoder.py:137,
+ * a maximum over every (frame, camera) of the call; here each frame b has its own
+ *   max_len_b = max over cams of counts[b][cam]   (counts [B][cams] as tt_look_project writes them; device memory, no host sync).
+ * tt_msda_forward_frames: tt_msda_forward computing only rows r < max_len_b of the images bn = b * cams + cam (d->BN = B * cams);
+ * the other rows of `out` are not written.  Never more rows than tt_msda_forward with the batch-wide max_len. */
+int tt_msda_forward_frames(const tt_msda_desc* d, const float* value, const float* off, const float* logits, const float* ref,
+                           const int* counts, int cams, float* out, tt_stream_t stream);
+/* msda:338-342 at B = 1 per frame: out[b][cam*C + c] = sum over 1 <= r < min(max_len_b, cap) of rows[b][cam][r][c] (row 0 zeroed,
+ * divisor 1).  Rows in [counts[b][cam], max_len_b) are the zero-query rows tt_look_rebatch wrote; they count, as in the reference. */
+int tt_look_reduce_frames(const float* rows, int B, int cams, int cap, int C, const int* counts, float* out,
+                          tt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (7) decoder glue

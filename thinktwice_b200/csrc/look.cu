@@ -3,7 +3,8 @@
 // The reference builds the rebatched queries with Python loops, `.nonzero()` and 4*B host syncs per
 // layer; here projection, ordered compaction, query assembly and the 4-level bilinear FPN gather run
 // on the device with the batch-wide max_len kept in a device scalar (no host round trip), and every
-// feature gather is a channel-contiguous (coalesced) read of a channels-last map.
+// feature gather is a channel-contiguous (coalesced) read of a channels-last map.  The *_frames entries bound and reduce
+// the rows of each frame by that frame's own max_len (independent frames: B = 1 semantics per frame).
 #include "common.cuh"
 
 extern long long g_tt_launches;
@@ -119,10 +120,26 @@ __global__ void __launch_bounds__(256) look_rebatch_kernel(
   }
 }
 
-// one warp per (row, head); lane = channel of the head (dh == 32) and, for the softmax, sample index
+// Row bound of one (frame, camera) image bn = b * cams + cam.  Batch-coupled (the reference's semantics at any B,
+// thinktwice_decoder.py:137): the batch-wide max_len, one device scalar.  Per frame (the reference run on frame b alone, B = 1):
+// the largest count over that frame's cameras, read from the counts tt_look_project wrote.
+enum RowBound { kBatchMaxLen, kFrameMaxLen };
+
+template <RowBound RB>
+TT_DEVICE int look_row_bound(const int* bound, int bn, int cams) {
+  if (RB == kBatchMaxLen) return *bound;
+  const int* c = bound + (bn / cams) * cams;
+  int ml = 0;
+  for (int i = 0; i < cams; ++i) ml = max(ml, c[i]);
+  return ml;
+}
+
+// one warp per (row, head); lane = channel of the head (dh == 32) and, for the softmax, sample index.  Rows at or past the
+// row bound of their image are not computed (bound NULL: every row).
+template <RowBound RB>
 __global__ void __launch_bounds__(256) msda_kernel(const tt_msda_desc d, const float* __restrict__ value,
                                                    const float* __restrict__ off, const float* __restrict__ logits,
-                                                   const float* __restrict__ ref, const int* __restrict__ max_len,
+                                                   const float* __restrict__ ref, const int* __restrict__ bound, int cams,
                                                    float* __restrict__ out) {
   const long long wid = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / 32;
   const int lane = threadIdx.x & 31;
@@ -131,7 +148,7 @@ __global__ void __launch_bounds__(256) msda_kernel(const tt_msda_desc d, const f
   if (row >= (long long)d.BN * d.rows_cap) return;
   const int r = row % d.rows_cap;
   const int bn = row / d.rows_cap;
-  if (max_len && r >= *max_len) return;
+  if (bound && r >= look_row_bound<RB>(bound, bn, cams)) return;
   const int S = d.levels * d.points;                        // 32 samples per head
   const int E = d.heads * d.dh;
   // softmax over the S logits of this head (msda:480-483)
@@ -170,15 +187,19 @@ __global__ void __launch_bounds__(256) msda_kernel(const tt_msda_desc d, const f
   if (lane < d.dh) out[row * E + head * d.dh + lane] = acc;
 }
 
+// msda:338-342 zeroes the first len(indexes[cam]) rows of every image and divides by it; that length is the number of frames
+// in the forward call (B when coupled, 1 for a frame on its own), and the sum runs up to the row bound.
+template <RowBound RB>
 __global__ void look_reduce_kernel(const float* __restrict__ rows, int B, int cams, int cap, int C,
-                                   const int* __restrict__ max_len, float* __restrict__ out) {
+                                   const int* __restrict__ bound, float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * cams * C) return;
   const int c = i % C, bn = i / C;
-  const int ml = min(*max_len, cap);
-  const float div = (float)(B > 1 ? B : 1);
+  const int ml = min(look_row_bound<RB>(bound, bn, cams), cap);
+  const int first = RB == kBatchMaxLen ? B : 1;
+  const float div = (float)(first > 1 ? first : 1);
   float s = 0.f;
-  for (int r = B; r < ml; ++r) s += rows[((long long)bn * cap + r) * C + c] / div;   // msda:338-342
+  for (int r = first; r < ml; ++r) s += rows[((long long)bn * cap + r) * C + c] / div;
   out[i] = s;
 }
 
@@ -219,15 +240,38 @@ int tt_msda_forward(const tt_msda_desc* d, const float* value, const float* off,
   TT_REQUIRE(d->dh == 32 && d->levels * d->points <= 32 && d->levels <= 4, "tt_msda_forward", "needs dh == 32, <= 32 samples");
   const long long warps = (long long)d->BN * d->rows_cap * d->heads;
   if (warps == 0) return TT_OK;
-  msda_kernel<<<tt_cdiv(warps * 32, 256), 256, 0, (cudaStream_t)stream>>>(*d, value, off, logits, ref, max_len, out);
+  msda_kernel<kBatchMaxLen><<<tt_cdiv(warps * 32, 256), 256, 0, (cudaStream_t)stream>>>(*d, value, off, logits, ref, max_len, 1, out);
   TT_LAUNCHED("tt_msda_forward");
+  return TT_OK;
+}
+
+int tt_msda_forward_frames(const tt_msda_desc* d, const float* value, const float* off, const float* logits, const float* ref,
+                           const int* counts, int cams, float* out, tt_stream_t stream) {
+  TT_REQUIRE(d && value && off && logits && ref && counts && out, "tt_msda_forward_frames", "null argument");
+  TT_REQUIRE(d->dh == 32 && d->levels * d->points <= 32 && d->levels <= 4, "tt_msda_forward_frames", "needs dh == 32, <= 32 samples");
+  TT_REQUIRE(cams > 0 && d->BN % cams == 0, "tt_msda_forward_frames", "BN must be a multiple of cams > 0");
+  const long long warps = (long long)d->BN * d->rows_cap * d->heads;
+  if (warps == 0) return TT_OK;
+  msda_kernel<kFrameMaxLen><<<tt_cdiv(warps * 32, 256), 256, 0, (cudaStream_t)stream>>>(*d, value, off, logits, ref, counts, cams, out);
+  TT_LAUNCHED("tt_msda_forward_frames");
   return TT_OK;
 }
 
 int tt_look_reduce(const float* rows, int B, int cams, int cap, int C, const int* max_len, float* out, tt_stream_t stream) {
   TT_REQUIRE(rows && max_len && out, "tt_look_reduce", "null argument");
-  look_reduce_kernel<<<tt_cdiv((long long)B * cams * C, 256), 256, 0, (cudaStream_t)stream>>>(rows, B, cams, cap, C, max_len, out);
+  look_reduce_kernel<kBatchMaxLen><<<tt_cdiv((long long)B * cams * C, 256), 256, 0, (cudaStream_t)stream>>>(rows, B, cams, cap, C,
+                                                                                                            max_len, out);
   TT_LAUNCHED("tt_look_reduce");
+  return TT_OK;
+}
+
+int tt_look_reduce_frames(const float* rows, int B, int cams, int cap, int C, const int* counts, float* out, tt_stream_t stream) {
+  TT_REQUIRE(rows && counts && out, "tt_look_reduce_frames", "null argument");
+  TT_REQUIRE(B >= 0 && cams > 0 && cap > 0 && C > 0, "tt_look_reduce_frames", "bad sizes");
+  if (B == 0) return TT_OK;
+  look_reduce_kernel<kFrameMaxLen><<<tt_cdiv((long long)B * cams * C, 256), 256, 0, (cudaStream_t)stream>>>(rows, B, cams, cap, C,
+                                                                                                            counts, out);
+  TT_LAUNCHED("tt_look_reduce_frames");
   return TT_OK;
 }
 

@@ -168,16 +168,40 @@ class EncoderDecoder(nn.Module):
         # staged into a buffer whose capacity is the count rounded up to POINT_BUCKET, the tail filled with
         # out-of-range points (dropped by the voxeliser exactly like any point outside point_cloud_range), so that one
         # arena and one CUDA graph serve every tick of a bucket.
-        pts = batch['points'][:, -1].to(torch.float32)
-        P = pts.shape[1]
+        # `points` is the collated (B, 1, P, 5) tensor, or a list of B per-frame (1, P_b, 5) clouds (several agents' ticks).
+        # A list is padded to its longest cloud: with zero points as mmcv's collate pads (batch-coupled mode: bitwise the
+        # collated tensor's result), or with out-of-range points in independent-frames mode, so that a short cloud gains no
+        # phantom voxel at the origin and its frame equals the frame run alone.  A collated tensor is taken as given in both
+        # modes: its zero rows are points.
+        clouds = batch['points']
+        ragged = isinstance(clouds, (list, tuple))
+        if ragged:
+            if len(clouds) != B:
+                raise ValueError(f"batch['points'] holds {len(clouds)} clouds for {B} frames")
+            clouds = [c[-1].to(torch.float32) for c in clouds]     # (1, P_b, 5) -> (P_b, 5)
+            P, F = max(c.shape[0] for c in clouds), clouds[0].shape[1]
+        else:
+            pts = clouds[:, -1].to(torch.float32)
+            P, F = pts.shape[1], pts.shape[2]
         cap = -(-P // POINT_BUCKET) * POINT_BUCKET
         mv = self.lidar_encoder.max_voxels
         if cap > mv >= P:                                          # tt_voxelize_mean wants points per frame <= max_voxels
             cap = mv
-        pb = e.buf('in.points', (B, cap, pts.shape[2]))
-        if cap != P:
-            e.fill(pb, 1e30)
-        pb[:, :P].copy_(pts, non_blocking=True)
+        pb = e.buf('in.points', (B, cap, F))
+        if not ragged:
+            if cap != P:
+                e.fill(pb, 1e30)
+            pb[:, :P].copy_(pts, non_blocking=True)
+        else:
+            independent = self.decoder.independent_frames
+            if cap != P or (independent and any(c.shape[0] < P for c in clouds)):
+                e.fill(pb, 1e30)
+            for b, c in enumerate(clouds):
+                n = c.shape[0]
+                if n:
+                    pb[b, :n].copy_(c, non_blocking=True)
+                if n < P and not independent:
+                    e.fill(pb[b, n:P], 0.0)                        # mmcv collate's zero padding
         e.cur['in.points'] = pb
         if mats:
             self.stage_mats(batch, B, T, N)
@@ -406,7 +430,7 @@ class EncoderDecoder(nn.Module):
         pipelined = (self.pipeline_uploads and not im0.is_cuda and (im0.dim() == 6 and im0.shape[1] > 1) and not warm and e.device.type == 'cuda'
                      and e.overlap and e.prof is None and e.marks is None)
         img, key = self.stage(batch, mats=not pipelined)
-        key = key + (warm,)
+        key = key + (warm, self.decoder.independent_frames)        # a graph is captured in one Look mode and replayed in it only
         T = img.shape[1]
         use_graph = getattr(self, 'use_graph', False)
         # Graph mode, first forward of a key: ONE eager pass computes this call's result (and allocates every persistent buffer), then the
@@ -458,7 +482,18 @@ class EncoderDecoder(nn.Module):
         return self
 
     def reset_stream(self):
+        """start a new stream for the streaming BEV cache.  The cache holds one key-frame BEV per frame of the batch and is reset as a
+        whole: when any agent of a batch starts an episode, call this; the next forward is one cold tick for the whole batch."""
         self.img_encoder.reset_stream()
+
+    def enable_independent_frames(self, flag=True):
+        """Look-module batch semantics.  Off (the default): the reference's, where the frames of one forward call are coupled (row bound
+        max_len over the whole batch, first B rows zeroed, divide by B: thinktwice_decoder.py:137, msda:338-342), so a frame's prediction
+        depends on the batch it is in.  On: every frame is computed as the reference computes it alone at B = 1 (the closed-loop agent's
+        batch), so a batch of several agents' frames, or a shard of one, predicts for each frame what it predicts alone.  At B = 1 the
+        two modes are the same computation.  CUDA graphs are captured per mode."""
+        self.decoder.independent_frames = bool(flag)
+        return self
 
     SMALL_OUTPUTS = ('pred_speed', 'pred_value_traj', 'pred_features_traj', 'pred_value_ctrl', 'pred_features_ctrl', 'pred_wp',
                      'mu_branches', 'sigma_branches', 'future_mu', 'future_sigma')

@@ -108,7 +108,7 @@ EXPORTS = [
     'tt_maxpool3x3s2', 'tt_upsample2x_bilinear_ac', 'tt_global_avgpool', 'tt_broadcast_rows', 'tt_se_gate', 'tt_se_pool',
     'tt_se_apply', 'tt_anti_transpose', 'tt_copy2d', 'tt_layernorm', 'tt_eltwise', 'tt_fill', 'tt_dcn_im2col',
     'tt_voxelize_workspace_bytes', 'tt_voxelize_mean', 'tt_rulebook_workspace_bytes', 'tt_sparse_rulebook',
-    'tt_sparse_conv', 'tt_sparse_to_bev', 'tt_conv2d_f16s', 'tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_pointwise_f16s', 'tt_upsample2x_bilinear_ac_split', 'tt_f16s_saturation_count', 'tt_sparse_conv_f16s', 'tt_sparse_conv_os_f16s', 'tt_look_project', 'tt_look_rebatch', 'tt_msda_forward', 'tt_look_reduce', 'tt_gru_input',
+    'tt_sparse_conv', 'tt_sparse_to_bev', 'tt_conv2d_f16s', 'tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_pointwise_f16s', 'tt_upsample2x_bilinear_ac_split', 'tt_f16s_saturation_count', 'tt_sparse_conv_f16s', 'tt_sparse_conv_os_f16s', 'tt_look_project', 'tt_look_rebatch', 'tt_msda_forward', 'tt_look_reduce', 'tt_msda_forward_frames', 'tt_look_reduce_frames', 'tt_gru_input',
     'tt_preprocess_u8', 'tt_lidar_stitch', 'tt_points_union', 'tt_voxel_pooling_backward', 'tt_ms_deform_attn_forward', 'tt_ms_deform_attn_backward',
 ]
 

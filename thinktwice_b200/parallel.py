@@ -3,8 +3,10 @@
 Frames of a batch are split into contiguous chunks, one per rank (one process per GPU); weights are replicated;
 after the forward ONE all-gather returns every rank's waypoints `(B_local, K+1, 4, 2)` — a few hundred bytes, i.e.
 a latency-bound NCCL call issued on the compute stream right after the last decoder kernel.  No kernel has a
-collective to fuse with.  NOTE (SURVEY fact 4): the reference's Look module couples the frames of one forward call,
-so sharded results equal the reference run with the SAME per-rank chunk, not the un-sharded batch.
+collective to fuse with.  NOTE (SURVEY fact 4): in the default mode the reference's Look module couples the frames of one
+forward call, so sharded results equal the reference run with the SAME per-rank chunk, not the un-sharded batch.  With
+`model.enable_independent_frames()` every frame is computed as if alone, so a sharded batch equals the un-sharded batch frame
+for frame.  A list of per-frame clouds in batch['points'] is sliced like the other per-frame lists.
 """
 import torch
 import torch.distributed as dist

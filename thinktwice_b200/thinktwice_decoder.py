@@ -3,8 +3,9 @@
 Mirror of open_loop_training/code/model_code/dense_heads/thinktwice_decoder.py:262-489 (forward only),
 with the Look module's SpatialCrossAttention / MSDeformableAttention3D
 (multi_scale_deformable_attn_function.py:216-526) and SpatialGRU (dense_heads/utils.py:53-106).
-Reference quirks kept bit-for-bit in semantics: batch-wide max_len, "zero the first B rows / divide by
-B" (msda:338-342).  Dead work is skipped with identical outputs: PredictionModule.ffn
+Reference quirks kept bit-for-bit in semantics by default: batch-wide max_len, "zero the first B rows / divide by
+B" (msda:338-342).  With `independent_frames` each frame gets B = 1 semantics instead (its own max_len, row 0 zeroed,
+divisor 1), so a frame predicts what it predicts alone.  Dead work is skipped with identical outputs: PredictionModule.ffn
 (thinktwice_decoder.py:44-46) and the LiDAR look branch (:179-186, replaced by zeros in the reference).
 """
 import ctypes as C
@@ -61,6 +62,7 @@ class ThinkTwiceDecoder(nn.Module):
         self.T = config['pred_len']
         self.K = config['refine_num']
         self.value_all_budget = 8 << 30     # bytes the merged value_proj output may take (else per-layer projection)
+        self.independent_frames = False     # Look module: batch-coupled reference semantics (False) or B = 1 per frame (True)
 
     # ------------------------------------------------------------------ weights
     def prepare(self, pk, eng, parent):
@@ -204,19 +206,25 @@ class ThinkTwiceDecoder(nn.Module):
                 e.conv(meta['fpn'][l], L['value'][l], out=out, name=f'look.value{l}', y_nstride=nk * 256, bias_n_mod=cams)
         off = e.linear(q, L['off'], name='look.off')
         aw = e.linear(q, L['aw'], name='look.aw')
-        # tt_msda_forward writes the first max_len rows of each (frame, camera) only; the FFN below runs over all `cap` rows (static
+        # tt_msda_forward writes the first max_len rows of each (frame, camera) only (tt_msda_forward_frames: max_len_b of its frame); the FFN below runs over all `cap` rows (static
         # shapes for graph replay) and tt_look_reduce reads the valid ones.  Zero-filled once, so that the rows no forward has written yet
         # hold zeros instead of stale memory, which look.ffn2's epilogue would split into fp16 planes and count as saturated
         att = e.fmap('look.att', B * cams * cap, 1, 1, 256, zero=True)
         md = meta['msda_desc']
         md.value_ld, md.value_coff = (self.K * 256, k * 256) if meta['value_all'] is not None else (0, 0)
-        lib.call('tt_msda_forward', C.byref(md), _p(value), _p(off.t), _p(aw.t), _p(ref_re), _p(max_len), _p(att.t))
+        if self.independent_frames:                                  # rows bounded by each frame's own max_len (from `counts`)
+            lib.call('tt_msda_forward_frames', C.byref(md), _p(value), _p(off.t), _p(aw.t), _p(ref_re), _p(counts), cams, _p(att.t))
+        else:
+            lib.call('tt_msda_forward', C.byref(md), _p(value), _p(off.t), _p(aw.t), _p(ref_re), _p(max_len), _p(att.t))
         # PositionwiseFeedForward (msda:197-214)
         h = e.layernorm(att, *L['ffn_ln'], name='look.ffn_ln')
         h = e.linear(h, L['ffn1'], name='look.ffn1', act=ACT_GELU)
         h = e.linear(h, L['ffn2'], name='look.ffn2', res=att)
         red = e.fmap('look.red', B, 1, 1, cams * 256)
-        lib.call('tt_look_reduce', _p(h.t), B, cams, cap, 256, _p(max_len), _p(red.t))
+        if self.independent_frames:
+            lib.call('tt_look_reduce_frames', _p(h.t), B, cams, cap, 256, _p(counts), _p(red.t))
+        else:
+            lib.call('tt_look_reduce', _p(h.t), B, cams, cap, 256, _p(max_len), _p(red.t))
         o = e.layernorm(red, *L['op_ln'], name='look.op_ln')
         o = e.linear(o, L['op1'], name='look.op1', act=ACT_GELU)
         return e.linear(o, L['op3'], name='look.img')                # (B, 256)
