@@ -38,8 +38,9 @@ const char* tt_last_error(void);
 long long tt_launch_count(void);
 /* diagnosis knobs for kernel micro-benchmarks (tools/conv_bench.py); 0 in normal operation.  128: no split-K in the tensor-core
  * convs; bits 8..15: SMs the persistent tensor-core kernels leave free; 0x20000 / 0x40000: register accumulator folded every 4 / 1
- * stages instead of 2; 0x200000: one tap per K slab in the output-stationary sparse conv; 0x400000: 64-column tiles for every dense
- * f16s conv (no 128-column tiles).  Unknown bits: TT_ERR_INVALID, nothing set. */
+ * stages instead of 2 (in the output-stationary sparse conv: every 4 / 1 executed stages, the taps a tile skips not counted);
+ * 0x200000: one tap per K slab in the output-stationary sparse conv; 0x400000: 64-column tiles for every dense f16s conv and every
+ * output-stationary sparse conv (no 128-column tiles).  Unknown bits: TT_ERR_INVALID, nothing set. */
 int tt_debug_set(int flags);
 
 /* ------------------------------------------------------------------------------------------

@@ -17,9 +17,10 @@
 //   spans 2 x 64 K elements.
 // Tiling follows gemm_conv_tc.cu: TMA box loads per tap (zero fill = padding, element strides = stride 2), persistent CTAs
 // (one per SM), split-K and GATHER (sparse convolution).
-// Warp roles: warpgroup 0 = producer (warp 0: TMA / gather; warps 1..3 idle);
-// warpgroups 1 and 2 = wgmma + epilogue for rows 0..63 / 64..127 of the tile.  The producer keeps 40 registers per thread (88 when
-// it gathers) and the MMA warpgroups take the rest (setmaxnreg), which lets a 128-column tile keep its 192 accumulators in registers.
+// Warp roles: warpgroup 0 = producer (dense: one TMA thread; tap-major sparse: warp 0 gathers; output-stationary sparse: all four
+// warps gather, one tile row per thread); warpgroups 1 and 2 = wgmma + epilogue for rows 0..63 / 64..127 of the tile.  The producer
+// keeps 40 registers per thread (88 for the tap-major gather) and the MMA warpgroups take the rest (setmaxnreg), which lets a
+// 128-column tile keep its 192 accumulators in registers.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -38,13 +39,18 @@ constexpr int BM = 128;           // M tile: two warpgroups x 64 rows
 constexpr int KE = 64;            // K elements per stage (one 128-byte swizzle row of halves)
 constexpr int NTHREADS = 384;     // warpgroup 0 producer, warpgroups 1..2 MMA + epilogue
 // registers per thread after setmaxnreg (a 384-thread CTA starts with 168): the TMA producer is one thread with a handful of
-// values; the gather producer (sparse modes) keeps row indices of several stages in flight and needs more
-template <bool GATHER> constexpr int reg_producer() { return GATHER ? 88 : 40; }
-template <bool GATHER> constexpr int reg_mma() { return GATHER ? 208 : 232; }
-static_assert(128 * reg_producer<false>() + 256 * reg_mma<false>() <= 168 * NTHREADS &&
-              128 * reg_producer<true>() + 256 * reg_mma<true>() <= 168 * NTHREADS, "setmaxnreg must not ask for more than the CTA holds");
+// values, and so is each thread of the output-stationary gather (one row, its indices in shared memory); the tap-major gather
+// (GM 1) keeps the row indices of its pair tile in registers and needs more
+template <int GM> constexpr int reg_producer() { return GM == 1 ? 88 : 40; }
+template <int GM> constexpr int reg_mma() { return GM == 1 ? 208 : 232; }
+static_assert(128 * reg_producer<0>() + 256 * reg_mma<0>() <= 168 * NTHREADS &&
+              128 * reg_producer<1>() + 256 * reg_mma<1>() <= 168 * NTHREADS, "setmaxnreg must not ask for more than the CTA holds");
 constexpr float LO_SCALE = 2048.f, LO_INV = 1.f / 2048.f;
 constexpr int MAX_KVOL = 32;
+// shared memory beyond the stage ring: 8 warp-private transposition slabs, barriers, the tap prefix (GM 1) and the per-stage tile
+// length and tap masks (GM 2); then, output-stationary only, the neighbour block of the current 128-row tile
+constexpr int EPI_BYTES = 8 * 16 * 20 * 4 + 512;
+constexpr int NB_BYTES = 128 * MAX_KVOL * 4;
 constexpr float H_MAX = 65504.f;
 
 TT_DEVICE void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3, int c4) {
@@ -117,8 +123,8 @@ struct HArgs {
 };
 
 // GM (gather mode): 0 = dense convolution (TMA box loads); 1 = tap-major sparse convolution (work item = one tap's pair tile,
-// red.add epilogue); 2 = output-stationary sparse convolution (work item = an output-row tile, K runs over ALL taps through the
-// neighbour table, plain fused epilogue — no atomics, no init / finish passes; pays for empty (row, tap) slots with zero rows).
+// red.add epilogue); 2 = output-stationary sparse convolution (work item = an output-row tile, K runs over the taps that some row
+// of the tile uses, through the neighbour table; plain fused epilogue — no atomics, no init / finish passes).
 template <int BN, int STAGES, int GM>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const HArgs p) {
@@ -135,17 +141,20 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   uint64_t* empty = bars + STAGES;                        // [STAGES]  MMA warps -> producer
   int* sp_first = reinterpret_cast<int*>(bars + 2 * STAGES);
   int* sp_cnt = sp_first + MAX_KVOL + 1;
+  int* tile_k = sp_cnt + MAX_KVOL;                        // [STAGES] output-stationary: K stages of the tile a stage belongs to
+  uint32_t* wmask = reinterpret_cast<uint32_t*>(tile_k + STAGES);                    // [4] per producer warp: taps its rows use
+  int* nb_s = reinterpret_cast<int*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);       // [BM][kvol] (GM == 2)
 
   const tt_conv_desc& d = p.d;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool GATHER = GM != 0;
-  const int taps = GM == 2 ? p.kvol : d.KH * d.KW;
-  // output-stationary with Cin = 32: a 64-half K slab holds TWO taps (p.tps = 2), so no half of a slab is padding
-  const int k_iters = (GM == 2 && p.tps == 2) ? (p.kvol + 1) / 2 : taps * p.n_slabs;
+  const int taps = d.KH * d.KW;
+  const int k_iters = taps * p.n_slabs;
   const int os_rows = GM == 2 ? min(*p.out_count, p.cap_rows) : 0;     // output-stationary: rows that exist (device count)
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GATHER ? 33 : 1); mbar_init(&empty[s], 8); }   // 8 MMA warps release a stage
+    // full: one arrival with the expected bytes + one cp.async arrival per gathering thread (GM 1: warp 0; GM 2: warps 0..3)
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], GM == 2 ? 129 : GM == 1 ? 33 : 1); mbar_init(&empty[s], 8); }   // 8 MMA warps release a stage
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (GM == 1 && threadIdx.x == 64) {
@@ -192,98 +201,107 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   };
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(reg_producer<GATHER>()));
-    if (warp == 0 && GATHER) {
-      // ===================================================================== gather producer (whole warp) + weight TMA
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(reg_producer<GM>()));
+    if (GM == 2) {
+      // ===================================================================== output-stationary gather (4 warps) + weight TMA
+      // Per tile: the tile's neighbour block [128 rows][kvol] goes to shared memory (rows at or past the device count read as -1:
+      // the table may hold stale rows of a larger cloud there), each of the 128 producer threads gathers one row, and the K walk
+      // visits only the K units that some row of the tile uses: taps, or tap pairs when two taps share a slab (Cin = 32).  The
+      // tile's stage count reaches the MMA warps through tile_k[stage], written before the stage's full barrier arrival.  A tile
+      // that uses no tap at all still runs one stage of zero rows, so that its epilogue writes bias + activation (+ residual).
+      // Shared-memory budget: one 16 KB neighbour block next to the 4-stage ring (BN 64) / 3-stage ring (BN 128), about 220 KB;
+      // a second block to prefetch the next tile's indices would cost a ring stage.  The block's loads are issued while the MMA
+      // warps still consume the previous tile's stages in flight.  They are coalesced plain loads rather than one bulk copy: the
+      // live part of the block ends at the device count, on any 4-byte boundary, and a bulk copy moves multiples of 16 bytes.
+      const int t = threadIdx.x, kv = p.kvol;
+      const int upb = p.tps == 2 ? 1 : 0;                    // K unit of tap k: k >> upb
+      const int spu = p.tps == 2 ? 1 : p.n_slabs;             // stages per K unit
       const uint32_t txb = 2 * B_BYTES;
       int ig = 0;
       for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
         int nt, mt, tap, count, kb, ke;
         decode(pt, nt, mt, tap, count, kb, ke);
         const int n0 = nt * BN;
-        const int* pin = GM == 1 ? p.pairs_in + (long long)tap * p.pair_cap : nullptr;
-        int rows[4];
-        int nxa[4] = {-1, -1, -1, -1}, nxb[4] = {-1, -1, -1, -1};   // neighbour indices of the next stage / tap (GM == 2)
-        if (GM == 1) {
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int m = mt * BM + lane + 32 * i;
-            rows[i] = m < count ? __ldg(pin + m) : -1;
+        asm volatile("bar.sync 1, 128;" ::: "memory");        // every producer thread is done with the previous block
+        const int lim = min(count - mt * BM, BM) * kv;
+        const int* nsrc = p.nbr + (long long)mt * BM * kv;
+        for (int i = t; i < BM * kv; i += 128) nb_s[i] = i < lim ? __ldg(nsrc + i) : -1;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        const int* my = nb_s + t * kv;                        // stride kvol (odd for 3^3 / 3 taps): conflict-free
+        uint32_t bits = 0;
+        for (int k = 0; k < kv; ++k) bits |= (my[k] >= 0 ? 1u : 0u) << (k >> upb);
+        bits = __reduce_or_sync(0xffffffffu, bits);
+        if (lane == 0) wmask[warp] = bits;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        uint32_t mask = wmask[0] | wmask[1] | wmask[2] | wmask[3];
+        const bool none = mask == 0;
+        const int nst = none ? 1 : __popc(mask) * spu;
+        if (none) mask = 1;
+        for (int j = 0, slab = 0; j < nst; ++j, ++ig) {
+          const int u = __ffs(mask) - 1;
+          const int s = ig % STAGES;
+          mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
+          uint8_t* st = smem + s * STAGE_BYTES;
+          if (t == 0) {
+            tile_k[s] = nst;
+            mbar_expect_tx(&full[s], txb);                   // (release: orders the tile_k store before the MMA warps' acquire)
+            // two taps per slab: weights viewed as [Cout][kvol * 32], K runs across the taps; else one tap's Cin per slab walk
+            if (upb) load_weights(st, &full[s], u * KE, 0, n0);
+            else load_weights(st, &full[s], slab * KE, u, n0);
           }
+          const uint32_t dst = smem_u32(st) + t * 128;
+          if (upb) {
+            // chunks 0..3 of the row come from the neighbour under tap 2 u, chunks 4..7 from tap 2 u + 1
+            const int ra = none ? -1 : my[2 * u], rb = (none || 2 * u + 1 >= kv) ? -1 : my[2 * u + 1];
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int row = jj < 4 ? ra : rb;
+              const bool ok = row >= 0;
+              const __half* src = p.gx + (long long)max(row, 0) * p.gx_ld + (jj & 3) * 8;
+              const uint32_t o = (uint32_t)((jj ^ (t & 7)) << 4);          // 16-byte chunk jj of row t lives at chunk jj ^ (t & 7)
+              cp_async16(dst + o, ok ? (const void*)src : (const void*)p.gx, ok ? 16 : 0);
+              cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane) : (const void*)p.gx, ok ? 16 : 0);
+            }
+          } else {
+            const int row = none ? -1 : my[u];
+            const int c0 = slab * KE;
+            const __half* src = p.gx + (long long)max(row, 0) * p.gx_ld + c0;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const bool ok = row >= 0 && c0 + jj * 8 < d.Cin;
+              const uint32_t o = (uint32_t)((jj ^ (t & 7)) << 4);
+              cp_async16(dst + o, ok ? (const void*)(src + jj * 8) : (const void*)p.gx, ok ? 16 : 0);
+              cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane + jj * 8) : (const void*)p.gx, ok ? 16 : 0);
+            }
+          }
+          cp_async_arrive_noinc(&full[s]);
+          if (++slab == spu) { slab = 0; mask &= mask - 1; }
+        }
+      }
+    } else if (warp == 0 && GM == 1) {
+      // ===================================================================== tap-major gather producer (whole warp) + weight TMA
+      const uint32_t txb = 2 * B_BYTES;
+      int ig = 0;
+      for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
+        int nt, mt, tap, count, kb, ke;
+        decode(pt, nt, mt, tap, count, kb, ke);
+        const int n0 = nt * BN;
+        const int* pin = p.pairs_in + (long long)tap * p.pair_cap;
+        int rows[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int m = mt * BM + lane + 32 * i;
+          rows[i] = m < count ? __ldg(pin + m) : -1;
         }
         for (int it = kb; it < ke; ++it, ++ig) {
           const int s = ig % STAGES;
-          if (GM == 2 && p.tps == 2) {
-            // ---- two taps per K slab (Cin = 32): chunks 0..3 of a row come from the neighbour under tap 2 it, chunks 4..7 from tap 2 it + 1
-            // (the neighbour indices of stage it + 1 are fetched while stage it's copies are issued)
-            int ra[4], rb[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (it == kb) {
-                const int m = mt * BM + lane + 32 * i;
-                const int* nb = p.nbr + (long long)m * p.kvol + 2 * it;
-                ra[i] = m < count ? __ldg(nb) : -1;
-                rb[i] = (m < count && 2 * it + 1 < p.kvol) ? __ldg(nb + 1) : -1;
-              } else {
-                ra[i] = nxa[i]; rb[i] = nxb[i];
-              }
-            }
-            if (it + 1 < ke) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int m = mt * BM + lane + 32 * i;
-                const int* nb = p.nbr + (long long)m * p.kvol + 2 * (it + 1);
-                nxa[i] = m < count ? __ldg(nb) : -1;
-                nxb[i] = (m < count && 2 * (it + 1) + 1 < p.kvol) ? __ldg(nb + 1) : -1;
-              }
-            }
-            mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
-            uint8_t* st = smem + s * STAGE_BYTES;
-            if (lane == 0) {
-              mbar_expect_tx(&full[s], txb);
-              load_weights(st, &full[s], it * KE, 0, n0);              // weights viewed as [Cout][kvol * 32]: K runs across the taps
-            }
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int r = lane + 32 * i;
-              const uint32_t dst = smem_u32(st) + r * 128;
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int row = j < 4 ? ra[i] : rb[i];
-                const bool ok = row >= 0;
-                const __half* src = p.gx + (long long)max(row, 0) * p.gx_ld + (j & 3) * 8;
-                const uint32_t o = (uint32_t)((j ^ (r & 7)) << 4);
-                cp_async16(dst + o, ok ? (const void*)src : (const void*)p.gx, ok ? 16 : 0);
-                cp_async16(dst + A_BYTES + o, ok ? (const void*)(src + p.gx_plane) : (const void*)p.gx, ok ? 16 : 0);
-              }
-            }
-            cp_async_arrive_noinc(&full[s]);
-            continue;
-          }
-          const int ktap = GM == 2 ? it / p.n_slabs : tap;            // output-stationary: the K walk visits every tap
-          const int slab = GM == 2 ? it - ktap * p.n_slabs : it;
-          if (GM == 2 && (slab == 0 || it == kb)) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int m = mt * BM + lane + 32 * i;
-              if (it == kb) rows[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap) : -1;       // -1: no input site under this tap
-              else rows[i] = nxa[i];                                                                       // fetched one tap ahead
-            }
-            if (ktap + 1 < taps) {                              // next tap's neighbours: in flight while this tap's copies are issued
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int m = mt * BM + lane + 32 * i;
-                nxa[i] = m < count ? __ldg(p.nbr + (long long)m * p.kvol + ktap + 1) : -1;
-              }
-            }
-          }
           mbar_wait(&empty[s], ((ig / STAGES) & 1) ^ 1);
           uint8_t* st = smem + s * STAGE_BYTES;
           if (lane == 0) {
             mbar_expect_tx(&full[s], txb);
-            load_weights(st, &full[s], slab * KE, ktap, n0);
+            load_weights(st, &full[s], it * KE, tap, n0);
           }
-          const int c0 = slab * KE;
+          const int c0 = it * KE;
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             const int r = lane + 32 * i;
@@ -337,7 +355,7 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
   } else {
     // ===================================================================== MMA + epilogue (warpgroups 1, 2)
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(reg_mma<GATHER>()));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(reg_mma<GM>()));
     const int cw = warp - 4;                                // MMA warp 0..7
     const int wg = cw >> 2;                                 // warpgroup: tile rows [64 wg, 64 wg + 64)
     const int row0 = wg * 64 + (cw & 3) * 16;               // this warp's 16 accumulator rows
@@ -350,6 +368,11 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     for (int pt = blockIdx.x; pt < total_items; pt += gridDim.x) {
       int nt, mt, tap, count, kb, ke;
       decode(pt, nt, mt, tap, count, kb, ke);
+      if (GM == 2) {                                         // the producer chose the tile's K walk: its length rides with stage 0
+        const int s = ig % STAGES;
+        mbar_wait(&full[s], (ig / STAGES) & 1);
+        ke = kb + tile_k[s];
+      }
       const int nch = (ke - kb + p.chunk - 1) / p.chunk;
       // ---- K walk: chunks of `chunk` stages accumulated by the tensor core, folded into fp32 sums with RN FMAs
       float sum[BN / 2];
@@ -750,18 +773,16 @@ __global__ void f16s_sparse_init_kernel(float* __restrict__ y, int y_ld, const f
   }
 }
 
-// shared memory beyond the stage ring: 8 warp-private transposition slabs, barriers and the tap prefix
-constexpr int EPI_BYTES = 8 * 16 * 20 * 4 + 512;
 // N tiles: each MMA thread holds BN / 2 main + BN / 2 correction accumulators plus BN / 2 fp32 sums, 96 registers at BN = 64 and
 // 192 at BN = 128 (within the 232 setmaxnreg gives the MMA warpgroups).  A BN = 128 stage is 64 KB, so its ring is 3 stages deep;
-// BN = 64 keeps 4 stages of 48 KB.  The sparse modes (GM 1 / 2) always use BN = 64.
+// BN = 64 keeps 4 stages of 48 KB.  The tap-major sparse mode (GM 1) always uses BN = 64.
 constexpr int BN_NARROW = 64, BN_WIDE = 128;
 
 // persistent grid: one CTA per SM walks the (M unit, N tile, K split) work items; debug bits 8..15: SMs left to a concurrent branch
 template <int BN, int GM>
 cudaError_t launch_f16s(const CUtensorMap& ma, const CUtensorMap& mb, const HArgs& a, long long m_units, cudaStream_t st) {
   constexpr int STAGES = BN == BN_WIDE ? 3 : 4;
-  constexpr int smem = STAGES * (2 * BM * KE * 2 + 2 * BN * KE * 2) + 1024 + EPI_BYTES;
+  constexpr int smem = STAGES * (2 * BM * KE * 2 + 2 * BN * KE * 2) + 1024 + EPI_BYTES + (GM == 2 ? NB_BYTES : 0);
   static_assert(smem <= 227 * 1024, "shared memory per block");
   static bool set = false;
   if (!set) { cudaFuncSetAttribute(conv_f16s_kernel<BN, STAGES, GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); set = true; }
@@ -1062,12 +1083,12 @@ int tt_sparse_conv_f16s(const tt_sparse_conv_desc* d, const void* feats_in_split
 int tt_sparse_conv_os_f16s(const tt_sparse_conv_desc* d, const tt_f16s_io* io, const int* nbr, const int* out_count, tt_stream_t stream) {
   TT_REQUIRE(d && io && io->x_split && io->w_split && (io->y || io->y_split) && nbr && out_count, "tt_sparse_conv_os_f16s", "null argument");
   TT_REQUIRE(!(io->res && io->res_split) && !io->res2 && !io->res2_split, "tt_sparse_conv_os_f16s", "one residual, fp32 or split planes");
-  if (d->Cin % 8 || d->Cout % 4 || d->in_ld % 8 || d->out_ld % 4 || d->Cin < 32 || d->Cout < 32 || d->kvol < 1 || io->x_plane % 8 || io->y_plane % 4 ||
+  if (d->Cin % 8 || d->Cout % 4 || d->in_ld % 8 || d->out_ld % 4 || d->Cin < 32 || d->Cout < 32 || d->kvol < 1 || d->kvol > MAX_KVOL || io->x_plane % 8 || io->y_plane % 4 ||
       (d->res_ld % 4) || io->res_plane % 4 ||
       ((reinterpret_cast<uintptr_t>(io->x_split) | reinterpret_cast<uintptr_t>(io->w_split) | reinterpret_cast<uintptr_t>(io->y) |
         reinterpret_cast<uintptr_t>(io->res) | reinterpret_cast<uintptr_t>(io->bias)) & 15) ||
       ((reinterpret_cast<uintptr_t>(io->y_split) | reinterpret_cast<uintptr_t>(io->res_split)) & 7)) {
-    tt_set_error("tt_sparse_conv_os_f16s: needs Cin %% 8, Cout %% 4, Cin / Cout >= 32, in_ld %% 8, out_ld %% 4, 16-byte aligned pointers");
+    tt_set_error("tt_sparse_conv_os_f16s: needs Cin %% 8, Cout %% 4, Cin / Cout >= 32, 1 <= kvol <= 32, in_ld %% 8, out_ld %% 4, 16-byte aligned pointers");
     return TT_ERR_UNSUPPORTED;
   }
   if (d->cap_out <= 0) return TT_OK;
@@ -1088,12 +1109,17 @@ int tt_sparse_conv_os_f16s(const tt_sparse_conv_desc* d, const tt_f16s_io* io, c
   a.gx = static_cast<const __half*>(io->x_split); a.gx_plane = io->x_plane; a.gx_ld = d->in_ld;
   a.kvol = d->kvol; a.nbr = nbr; a.out_count = out_count; a.cap_rows = d->cap_out;
   a.tps = (d->Cin == 32 && !(g_tt_debug & 0x200000)) ? 2 : 1;
-  a.splits = 1; a.k_per = a.tps == 2 ? (d->kvol + 1) / 2 : d->kvol * a.n_slabs;
-  a.n_tiles = tt_cdiv(d->Cout, BN_NARROW);
+  a.splits = 1; a.k_per = 1;                                      // (the kernel sizes each tile's K walk from its taps)
+  // 128-column tiles for Cout >= 128: one gather of the tile's rows feeds all 128 output columns instead of being repeated by a
+  // second 64-column work item.  Debug bit 0x400000 forces BN = 64 here too.
+  const bool wide = d->Cout >= BN_WIDE && !(g_tt_debug & 0x400000);
+  const int bn = wide ? BN_WIDE : BN_NARROW;
+  a.n_tiles = tt_cdiv(d->Cout, bn);
   CUtensorMap mb;
-  if (!encode_weights(&mb, io->w_split, d->Cin, d->kvol, d->Cout, BN_NARROW, a.tps == 2)) return TT_ERR_CUDA;
+  if (!encode_weights(&mb, io->w_split, d->Cin, d->kvol, d->Cout, bn, a.tps == 2)) return TT_ERR_CUDA;
   const long long cap_units = tt_cdiv(d->cap_out, BM);
-  const cudaError_t lerr = launch_f16s<BN_NARROW, 2>(mb, mb, a, cap_units, (cudaStream_t)stream);
+  const cudaError_t lerr = wide ? launch_f16s<BN_WIDE, 2>(mb, mb, a, cap_units, (cudaStream_t)stream)
+                                : launch_f16s<BN_NARROW, 2>(mb, mb, a, cap_units, (cudaStream_t)stream);
   if (lerr != cudaSuccess) { tt_set_error("tt_sparse_conv_os_f16s: launch failed: %s", cudaGetErrorString(lerr)); return TT_ERR_CUDA; }
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_sparse_conv_os_f16s");
