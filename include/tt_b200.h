@@ -205,7 +205,8 @@ int tt_copy2d(const float* src, int src_ld, float* dst, int dst_ld, int rows, in
 /* LayerNorm over the last dim (eps 1e-5), rows x D, output stride y_ld */
 int tt_layernorm(const float* x, int x_ld, const float* gamma, const float* beta, float* y, int y_ld, int rows,
                  int D, const int* row_count, tt_stream_t stream);
-/* elementwise: op 0: y = a + b; 1: y = (1 - a) * b; 2: y = (1 - a) * b + a * c; 3: y = act(a) */
+/* elementwise: op 0: y = a + b; 1: y = (1 - a) * b; 2: y = (1 - a) * b + a * c; 3: y = act(a);
+ * 4: y = act(a + log(-expm1(-a))), the inverse of softplus (thinktwice_decoder.py:22-23; a > 0) */
 int tt_eltwise(int op, int act, const float* a, int a_ld, const float* b, int b_ld, const float* c, int c_ld, float* y,
                int y_ld, int rows, int cols, tt_stream_t stream);
 int tt_fill(float* y, float v, long long n, tt_stream_t stream);
@@ -402,6 +403,40 @@ int tt_ms_deform_attn_forward(const tt_msda_desc* d, const float* value, const f
 int tt_ms_deform_attn_backward(const tt_msda_desc* d, const float* value, const float* sampling_loc, const float* attn_weight,
                                const float* grad_output, float* grad_value, float* grad_sampling_loc, float* grad_attn_weight,
                                tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (10) open-loop validation losses (thinktwice_decoder.py:536-620): every term of ThinkTwiceDecoder.loss in ONE launch.
+ * A term reduces an element-wise function of (pred, gt) over a logical tensor of up to 6 dims, each operand addressed by ELEMENT
+ * strides (0 = broadcast along that dim), so channels-last arena maps are read against NCHW ground truth without a copy.
+ */
+#define TT_LOSS_MAX_DIM 6
+enum {
+  TT_LOSS_SMOOTH_L1 = 0,        /* F.smooth_l1_loss, beta 1 */
+  TT_LOSS_SMOOTH_L1_CLAMP = 1,  /* clamp(smooth_l1(.), -5, 5) element-wise, then the mean (NaN stays NaN, as torch.clamp) */
+  TT_LOSS_L1 = 2,               /* |pred - gt| */
+  TT_LOSS_BETA_KL = 3,          /* kl_divergence(Beta(gt, gt2), Beta(pred, pred2)) in fp64; NaN unless all four are finite and > 0 */
+  TT_LOSS_ACTION_L1 = 4         /* |_get_action_beta(pred, pred2) - _get_action_beta(gt, gt2)| of component `aux` (framework:623-636) */
+};
+typedef struct {
+  const float* pred;            /* BETA_KL / ACTION_L1: alpha of the prediction */
+  const float* pred2;           /* BETA_KL / ACTION_L1: beta of the prediction (strides of pred); otherwise unused */
+  const float* gt;              /* NULL: a zero target */
+  const float* gt2;             /* BETA_KL / ACTION_L1: beta of the target (strides of gt) */
+  long long shape[TT_LOSS_MAX_DIM];
+  long long pred_stride[TT_LOSS_MAX_DIM];
+  long long gt_stride[TT_LOSS_MAX_DIM];
+  int ndim;                     /* 1 .. TT_LOSS_MAX_DIM */
+  int kind;                     /* TT_LOSS_* */
+  int slot;                     /* output slot: terms sharing a slot are added in term order */
+  int aux;                      /* ACTION_L1: the action component (0 throttle / brake, 1 steer) */
+  double scale;                 /* weight / element count: the term contributes scale * sum of its elements */
+} tt_loss_term;
+/* out[s] (fp32) = sum over the terms t with slot s, in term order, of terms[t].scale * (fp64 sum of t's elements).  Each term is
+ * split into a fixed number of element ranges, each range reduced in a fixed order by one CTA, and the last CTA to finish adds the
+ * range sums in a fixed order: two calls on the same inputs give bitwise equal results.  `terms` is HOST memory (copied into ws
+ * on `stream`); ws: tt_loss_workspace_bytes(n_terms) bytes of device memory, not shared with a concurrent call. */
+size_t tt_loss_workspace_bytes(int n_terms);
+int tt_loss_reduce(const tt_loss_term* terms, int n_terms, float* out, int n_slots, void* ws, size_t ws_bytes, tt_stream_t stream);
 
 #ifdef __cplusplus
 }

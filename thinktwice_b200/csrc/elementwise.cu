@@ -215,6 +215,7 @@ __global__ void eltwise_kernel(int op, int act, const float* __restrict__ a, int
       case 0: v = av + b[r * b_ld + col]; break;
       case 1: v = (1.f - av) * b[r * b_ld + col]; break;
       case 2: v = (1.f - av) * b[r * b_ld + col] + av * c[r * c_ld + col]; break;
+      case 4: v = av + logf(-expm1f(-av)); break;               // inverse softplus (thinktwice_decoder.py:22-23)
       default: v = av; break;
     }
     y[r * y_ld + col] = tt_act(v, act);
@@ -358,8 +359,8 @@ int tt_layernorm(const float* x, int x_ld, const float* gamma, const float* beta
 
 int tt_eltwise(int op, int act, const float* a, int a_ld, const float* b, int b_ld, const float* c, int c_ld, float* y,
                int y_ld, int rows, int cols, tt_stream_t stream) {
-  TT_REQUIRE(a && y && op >= 0 && op <= 3, "tt_eltwise", "bad arguments");
-  TT_REQUIRE(op == 3 || b, "tt_eltwise", "operand b missing");
+  TT_REQUIRE(a && y && op >= 0 && op <= 4, "tt_eltwise", "bad arguments");
+  TT_REQUIRE(op >= 3 || b, "tt_eltwise", "operand b missing");
   TT_REQUIRE(op != 2 || c, "tt_eltwise", "operand c missing");
   const long long total = (long long)rows * cols;
   if (total == 0) return TT_OK;

@@ -6,7 +6,7 @@ same registry name, same constructor keywords, same `forward_inference(batch)` /
 calls it unchanged.  The forward runs entirely in libtt_b200 (no eager / CPU fallback).
 """
 import time
-from collections import deque
+from collections import OrderedDict, deque
 
 import numpy as np
 import torch
@@ -506,16 +506,82 @@ class EncoderDecoder(nn.Module):
             pred[k] = pred[k].clone()
         return pred
 
+    SUPERVISION_KEYS = ('waypoints', 'action_mu', 'action_sigma', 'future_action_mu', 'future_action_sigma', 'value', 'feature',
+                        'grid_feature', 'future_grid_feature')
+
     def forward(self, is_eval=True, return_loss=False, **kwargs):
         """Reference signature (framework:393-407: `forward(is_eval=True, **kwargs)` with the batch as keywords).
-        The reference body always evaluates the training losses (`forward_train` + `_parse_losses`); losses and their
-        teacher-forcing inputs are out of this path's scope (SURVEY §8f, f4).  What IS on the path — the network forward
-        over the batch — runs here: the keywords are taken as the batch dict of `forward_inference`, and the result comes
-        back in the reference's output dict shape with the predictions attached and no loss."""
+        A batch that carries the supervision (`waypoints`, `action_mu`, ... as the training / validation loaders collate them) is
+        evaluated as the reference does it: forward_train + _parse_losses -> dict(loss, log_vars, num_samples), the open-loop
+        validation path of CustomEvalHook.  Losses are values: no gradients flow.  A batch without supervision is taken as the batch
+        dict of `forward_inference`, and the result comes back in the reference's output dict shape with the predictions attached
+        and no loss."""
+        if all(k in kwargs for k in self.SUPERVISION_KEYS):
+            loss, log_vars = self._parse_losses(self.forward_train(kwargs))
+            return dict(loss=loss, log_vars=log_vars, num_samples=self._batch_images(kwargs).shape[0])
         if return_loss:
-            raise NotImplementedError('losses / teacher forcing belong to the training path (SURVEY.md §8f f4)')
+            raise NotImplementedError('losses need the supervision keys in the batch: ' + ', '.join(self.SUPERVISION_KEYS))
         pred = self.forward_inference(kwargs)
         return dict(loss=None, log_vars={}, num_samples=self._batch_images(kwargs).shape[0], pred=pred)
+
+    @torch.no_grad()
+    def forward_train(self, batch):
+        """framework:147-191: the network over both sweeps, the decoder with teacher forcing, ThinkTwiceDecoder.loss.  The camera
+        branch's depth / segmentation supervision (train_cfg use_depth / use_seg) is not built: such a model raises.  Runs eagerly on
+        the inference arena without touching its CUDA graphs; a validation batch is not the next closed-loop tick, so the streaming
+        BEV cache starts over afterwards."""
+        cfg = self.config
+        missing = [n for n, k in (('depth_loss', 'use_depth'), ('seg_loss', 'use_seg')) if k in cfg and cfg[k]]
+        if missing:
+            raise NotImplementedError(f'{" and ".join(missing)} (train_cfg use_depth / use_seg) are not built yet: set them False to '
+                                      'evaluate the decoder losses')
+        if self.eng is None:
+            im0 = self._batch_images(batch)
+            self.prepare(im0.device if im0.is_cuda else 'cuda:0')
+        e = self.eng
+        B_now = self._batch_images(batch).shape[0]
+        if getattr(self, '_arena_B', B_now) != B_now:
+            self.release_buffers()
+        self._arena_B = B_now
+        self.img_encoder.reset_stream()
+        img, _ = self.stage(batch)
+        for t in range(img.shape[1]):
+            self._stage_sweep(img, t)
+        with e.side_branch() as side:
+            lidar = self._phase_lidar()
+        self._phase_history()
+        cam, meas = self._phase_key()
+        side.join()
+        flat, bev32, mid, lidar_hi = self.get_fusion_feat(cam['bev'], lidar[0])
+        teacher = {k: batch[k] for k in ('waypoints', 'action_sigma', 'action_mu', 'future_action_sigma', 'future_action_mu')}
+        pred = self.decoder(flat, bev32, meas, None, self, teacher, [None, None, cam['fpn_feats'], lidar_hi])
+        losses = self.decoder.loss(batch, pred, mid)
+        self.img_encoder.reset_stream()
+        self.last_cam_feat = cam
+        self.last_train = dict(pred=pred, mid=mid, flat=flat, bev32=bev32, meas=meas, lidar_hi=lidar_hi)   # for parity checks
+        return losses
+
+    @staticmethod
+    def _parse_losses(losses):
+        """framework:409-440: log_vars = the mean of every entry, loss = the sum of the entries whose name contains 'loss'; with
+        torch.distributed initialised every logged value is averaged over the ranks."""
+        import torch.distributed as dist
+        log_vars = OrderedDict()
+        for name, value in losses.items():
+            if isinstance(value, torch.Tensor):
+                log_vars[name] = value.mean()
+            elif isinstance(value, list):
+                log_vars[name] = sum(v.mean() for v in value)
+            else:
+                raise TypeError(f'{name} is not a tensor or list of tensors')
+        loss = sum(v for k, v in log_vars.items() if 'loss' in k)
+        log_vars['loss'] = loss
+        for name, value in log_vars.items():
+            if dist.is_available() and dist.is_initialized():
+                value = value.data.clone()
+                dist.all_reduce(value.div_(dist.get_world_size()))
+            log_vars[name] = value.item()
+        return loss, log_vars
 
     def forward_test(self, **kwargs):
         """mmdet-style test entry: the batch as keywords -> pred dict."""

@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(_HERE, 'libtt_b200.so')
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SIGMOID, ACT_SOFTPLUS, ACT_SOFTPLUS_CLAMP = 0, 1, 2, 3, 4, 5
 RES_NONE, RES_SAME, RES_UP2 = 0, 1, 2
 IMPL_AUTO, IMPL_SIMT, IMPL_TF32, IMPL_3XTF32, IMPL_F16S = 0, 1, 2, 3, 4
+ELT_INV_SOFTPLUS = 4            # tt_eltwise op: y = act(a + log(-expm1(-a)))
+LOSS_SMOOTH_L1, LOSS_SMOOTH_L1_CLAMP, LOSS_L1, LOSS_BETA_KL, LOSS_ACTION_L1 = 0, 1, 2, 3, 4
+LOSS_MAX_DIM = 6
 
 
 class TTError(RuntimeError):
@@ -79,6 +82,13 @@ class PreprocDesc(C.Structure):
                [(n, C.c_int) for n in ('pad_H', 'pad_W', 'pad_top', 'pad_left')]
 
 
+class LossTerm(C.Structure):
+    """tt_loss_term (include/tt_b200.h section 10): one term of tt_loss_reduce."""
+    _fields_ = [('pred', C.c_void_p), ('pred2', C.c_void_p), ('gt', C.c_void_p), ('gt2', C.c_void_p),
+                ('shape', C.c_longlong * LOSS_MAX_DIM), ('pred_stride', C.c_longlong * LOSS_MAX_DIM), ('gt_stride', C.c_longlong * LOSS_MAX_DIM),
+                ('ndim', C.c_int), ('kind', C.c_int), ('slot', C.c_int), ('aux', C.c_int), ('scale', C.c_double)]
+
+
 _lib = None
 
 
@@ -94,7 +104,7 @@ def load():
     lib.tt_last_error.restype = C.c_char_p
     lib.tt_launch_count.restype = C.c_longlong
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
-              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes'):
+              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -110,7 +120,21 @@ EXPORTS = [
     'tt_voxelize_workspace_bytes', 'tt_voxelize_mean', 'tt_rulebook_workspace_bytes', 'tt_sparse_rulebook',
     'tt_sparse_conv', 'tt_sparse_to_bev', 'tt_conv2d_f16s', 'tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_pointwise_f16s', 'tt_upsample2x_bilinear_ac_split', 'tt_f16s_saturation_count', 'tt_sparse_conv_f16s', 'tt_sparse_conv_os_f16s', 'tt_look_project', 'tt_look_rebatch', 'tt_msda_forward', 'tt_look_reduce', 'tt_msda_forward_frames', 'tt_look_reduce_frames', 'tt_gru_input',
     'tt_preprocess_u8', 'tt_lidar_stitch', 'tt_points_union', 'tt_voxel_pooling_backward', 'tt_ms_deform_attn_forward', 'tt_ms_deform_attn_backward',
+    'tt_loss_workspace_bytes', 'tt_loss_reduce',
 ]
+
+
+def pack_loss_terms(terms):
+    """list of term dicts (LossTerm's field names; pointers from `_p`) -> the tt_loss_term array tt_loss_reduce reads."""
+    arr = (LossTerm * len(terms))()
+    for a, t in zip(arr, terms):
+        if len(t['shape']) > LOSS_MAX_DIM:
+            raise TTError(f'loss term of {len(t["shape"])} dims (at most {LOSS_MAX_DIM})')
+        a.pred, a.pred2, a.gt, a.gt2 = t['pred'], t['pred2'], t['gt'], t['gt2']
+        a.ndim, a.kind, a.slot, a.aux, a.scale = len(t['shape']), t['kind'], t['slot'], t['aux'], t['scale']
+        for d, (n, ps, gs) in enumerate(zip(t['shape'], t['pred_stride'], t['gt_stride'])):
+            a.shape[d], a.pred_stride[d], a.gt_stride[d] = n, ps, gs
+    return arr
 
 
 def _stream():

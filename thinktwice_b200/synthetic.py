@@ -89,3 +89,31 @@ def make_batch(cfg, batch_size=1, seed=0, num_points=40000, device='cpu'):
     )
     batch['target_command_raw'] = batch['target_command'].argmax(-1)
     return batch
+
+
+def make_supervision(cfg, batch_size=1, seed=0, device='cpu'):
+    """Seeded ground truth in the reference's training-batch contract (the keys ThinkTwiceDecoder.loss and the teacher-forced pass
+    read, thinktwice_decoder.py:496-619): waypoints (B, T, 2); Beta parameters action_mu / action_sigma (B, 2) and T future ones
+    (lists of (B, 2)), drawn from U(0.5, 20) independently of any prediction so that no loss term is near zero; value (B,); the
+    flattened feature (B, 256); the BEV pyramid targets grid_feature = [None, None, 32x21x21, 64x10x10, 128x4x4, 256x2x2] and T
+    future 21x21 targets future_grid_feature[t] = [None, None, 32x21x21].  One generator per frame, as make_batch."""
+    T = cfg.model.train_cfg['pred_len']
+    shapes = {2: (32, 21, 21), 3: (64, 10, 10), 4: (128, 4, 4), 5: (256, 2, 2)}
+    frames = []
+    for j in range(batch_size):
+        g = torch.Generator().manual_seed(5000 + 1000 * seed + j)
+        beta = lambda *s: 0.5 + 19.5 * torch.rand(*s, generator=g)
+        f = dict(waypoints=torch.cumsum(torch.stack([1.0 + 2.0 * torch.rand(T, generator=g), 0.5 * torch.randn(T, generator=g)], -1), 0),
+                 action_mu=beta(2), action_sigma=beta(2), future_action_mu=beta(T, 2), future_action_sigma=beta(T, 2),
+                 value=torch.randn(1, generator=g), feature=torch.rand(256, generator=g))
+        for i, s in shapes.items():
+            f[f'grid{i}'] = 2.0 * torch.rand(*s, generator=g)
+        f['future_grid'] = 2.0 * torch.rand(T, *shapes[2], generator=g)
+        frames.append(f)
+    st = lambda k: torch.stack([f[k] for f in frames]).to(device)
+    grid = [None, None] + [st(f'grid{i}') for i in shapes]
+    fut = st('future_grid')
+    return dict(waypoints=st('waypoints'), action_mu=st('action_mu'), action_sigma=st('action_sigma'),
+                future_action_mu=list(st('future_action_mu').unbind(1)), future_action_sigma=list(st('future_action_sigma').unbind(1)),
+                value=st('value').view(-1), feature=st('feature'), grid_feature=grid,
+                future_grid_feature=[[None, None, fut[:, t]] for t in range(T)])
