@@ -16,7 +16,7 @@ def tt_msda_forward_frames(emu, d, value, off, logits, ref, counts, cams, out, s
     dd = _desc(d)
     BN, cap, E = dd.BN, dd.rows_cap, dd.heads * dd.dh
     assert cams > 0 and BN % cams == 0
-    full = torch.empty(BN * cap * E)
+    full = torch.empty(BN * cap * E, dtype=out.t.dtype, device=out.t.device)
     emu.tt_msda_forward(d, value, off, logits, ref, NULL, Ptr(full), stream)
     src, dst = full.view(BN, cap, E), out.flat()[:BN * cap * E].view(BN, cap, E)
     for b, ml in enumerate(frame_max_len(counts, BN // cams, cams)):

@@ -87,6 +87,93 @@ def _pix_view(p, N, H, W, ld, nstride=0, hstride=0, C=None):
     return torch.as_strided(p.flat(), (N, H, W, C if C is not None else ld), (ns, hs, ld, 1))
 
 
+def conv_ref(d, x, w, bias, res, res2, f16s=None, kmajor_w=False, magnitude=False):
+    """include/tt_b200.h (2) / (2b) in fp64 on the operands' device: (value, magnitude), both (N, OH, OW, Cout).  value =
+    act(conv(x, w) + bias + res + res2) from exactly what the kernel reads (split operands decoded as hi + lo' / 2048);
+    magnitude (only when asked, else None) = conv(|x|, |w|) + |bias| + |res| + |res2|, the pre-activation scale a rounding
+    bound is proportional to."""
+    taps = d.KH * d.KW
+    cg = d.Cin // d.groups
+    dev = (x.t if x else w.t).device
+
+    def xview(C_):                                                     # (N, H, W, C_) fp64 view of the input
+        Wv = d.W if C_ == d.Cin else d.x_hstride // d.x_ld
+        if f16s is None:
+            return _pix_view(x, d.N, d.H, Wv, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
+        hi = _pix_view(x, d.N, d.H, Wv, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
+        lo = _pix_view(Ptr(x.t, x.off + f16s.x_plane), d.N, d.H, Wv, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
+        return hi + lo / 2048.0
+    if f16s is not None and not kmajor_w:                              # [2][Cout][taps][Cin8] scaled-split half planes
+        c8 = -(-d.Cin // 8) * 8
+        planes = w.flat()[:2 * d.Cout * taps * c8].view(2, d.Cout, taps, c8).double()
+        wt = (planes[0] + planes[1] / 2048.0)[..., :d.Cin].reshape(d.Cout, d.KH, d.KW, d.Cin).permute(0, 3, 1, 2)
+        assert d.groups == 1
+    elif d.impl >= 2 and not kmajor_w:                                 # [2][Cout][taps][Cin] hi / lo planes
+        planes = w.flat()[:2 * d.Cout * taps * d.Cin].view(2, d.Cout, taps, d.Cin).double()
+        wt = (planes[0] + planes[1]).view(d.Cout, d.KH, d.KW, d.Cin).permute(0, 3, 1, 2)
+        assert d.groups == 1
+    else:                                                              # [taps * Cin_g][Cout]
+        wt = w.flat()[:taps * cg * d.Cout].view(d.KH, d.KW, cg, d.Cout).permute(3, 2, 0, 1).double()
+    if d.x_ld < d.Cin:                                                 # row-packed input: channels run on into the next pixels
+        assert d.KW == 1 and d.pad == 0 and d.groups == 1
+        px = d.Cin // d.x_ld                                           # pixels per K slab
+        xin = xview(d.x_ld).permute(0, 3, 1, 2)
+        wt = wt.reshape(d.Cout, px, d.x_ld, d.KH).permute(0, 2, 3, 1)                      # (Cout, c, kh, kw)
+        contract = lambda a, b: F.conv2d(a, b, stride=d.stride)
+    else:
+        xin = xview(d.Cin).permute(0, 3, 1, 2)
+        contract = lambda a, b: F.conv2d(a, b, stride=d.stride, padding=d.pad, dilation=d.dil, groups=d.groups)
+
+    def terms(f):                                                      # the summands of the epilogue, f = identity or abs
+        out = contract(f(xin), f(wt))
+        assert out.shape[2] >= d.OH and out.shape[3] >= d.OW, (tuple(out.shape), d.OH, d.OW)
+        out = out[..., :d.OH, :d.OW].permute(0, 2, 3, 1)               # (N, OH, OW, Cout)
+        if bias:
+            if d.bias_n_mod:
+                tab = bias.flat()[:d.bias_n_mod * d.Cout].view(d.bias_n_mod, d.Cout).double()
+                out = out + f(tab[torch.arange(d.N, device=dev) % d.bias_n_mod][:, None, None, :])
+            else:
+                out = out + f(bias.flat()[:d.Cout].double())
+        rs_, rp_ = (f16s.res_split, f16s.res_plane) if f16s is not None else (NULL, 0)
+        r2s_, r2p_ = (f16s.res2_split, f16s.res2_plane) if f16s is not None else (NULL, 0)
+        if d.res_mode == 1:
+            out = out + f(_res_view(d, res, rs_, rp_, d.N, d.OH, d.OW, d.res_ld, d.res_coff))
+        elif d.res_mode == 2:                                          # nearest-upsampled residual (PAFPN top-down)
+            r = _res_view(d, res, rs_, rp_, d.N, d.res_H, d.res_W, d.res_ld, d.res_coff)
+            ih = (torch.arange(d.OH, device=dev) * d.res_H) // d.OH
+            iw = (torch.arange(d.OW, device=dev) * d.res_W) // d.OW
+            out = out + f(r[:, ih][:, :, iw])
+        if res2 or r2s_:
+            out = out + f(_res_view(d, res2, r2s_, r2p_, d.N, d.OH, d.OW, d.res2_ld, d.res2_coff))
+        return out
+    return _act(terms(lambda v: v), d.act), (terms(torch.abs) if magnitude else None)
+
+
+def _res_view(d, p32, psplit, plane, N_, H_, W_, ld_, coff_):
+    """(N_, H_, W_, Cout) fp64 residual, from fp32 or from split planes."""
+    if p32:
+        return _pix_view(p32, N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
+    hi = _pix_view(psplit, N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
+    lo = _pix_view(Ptr(psplit.t, psplit.off + plane), N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
+    return hi + lo / 2048.0
+
+
+def y_region(d, p):
+    """the (N, OH, OW, Cout) elements of a conv output buffer (fp32 or one split plane, pointer p) that output rows go to."""
+    yv = _pix_view(p, d.N, d.yH, d.yW, d.y_ld, d.y_nstride, 0, d.Cout + d.y_coff)[..., d.y_coff:]
+    return yv[:, d.oy_add::d.oy_mul, d.ox_add::d.ox_mul][:, :d.OH, :d.OW]
+
+
+def conv_store(d, y, y_split, y_plane, out):
+    """write the fp32 result `out` (N, OH, OW, Cout) to y and / or the split planes, as the conv epilogue does."""
+    if y:
+        y_region(d, y)[...] = out
+    if y_split:
+        hi, lo = _split_f16(out)
+        for plane, val in ((0, hi), (y_plane, lo)):
+            y_region(d, Ptr(y_split.t, y_split.off + plane))[...] = val
+
+
 class Emu:
     def __init__(self):
         self.launches = 0
@@ -114,71 +201,8 @@ class Emu:
         d = _desc(d)
         self.launches += 1
         assert not gather and not m_count
-        taps = d.KH * d.KW
-        cg, og = d.Cin // d.groups, d.Cout // d.groups
-
-        def xview(C_):                                                 # (N, H, W, C_) fp64 view of the input
-            if f16s is None:
-                return _pix_view(x, d.N, d.H, d.W if C_ == d.Cin else d.x_hstride // d.x_ld, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
-            Wv = d.W if C_ == d.Cin else d.x_hstride // d.x_ld
-            hi = _pix_view(x, d.N, d.H, Wv, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
-            lo = _pix_view(Ptr(x.t, x.off + f16s.x_plane), d.N, d.H, Wv, d.x_ld, d.x_nstride, d.x_hstride, C_).double()
-            return hi + lo / 2048.0
-        xin = xview(d.Cin).permute(0, 3, 1, 2) if d.x_ld >= d.Cin else None
-        if f16s is not None and not kmajor_w:                          # [2][Cout][taps][Cin8] scaled-split half planes
-            c8 = -(-d.Cin // 8) * 8
-            planes = w.flat()[:2 * d.Cout * taps * c8].view(2, d.Cout, taps, c8).double()
-            wt = (planes[0] + planes[1] / 2048.0)[..., :d.Cin].reshape(d.Cout, d.KH, d.KW, d.Cin).permute(0, 3, 1, 2)
-            assert d.groups == 1
-        elif d.impl >= 2:                                              # [2][Cout][taps][Cin] hi / lo planes
-            planes = w.flat()[:2 * d.Cout * taps * d.Cin].view(2, d.Cout, taps, d.Cin).double()
-            wt = (planes[0] + planes[1]).view(d.Cout, d.KH, d.KW, d.Cin).permute(0, 3, 1, 2)
-            assert d.groups == 1
-        else:                                                          # [taps * Cin_g][Cout]
-            wt = w.flat()[:taps * cg * d.Cout].view(d.KH, d.KW, cg, d.Cout).permute(3, 2, 0, 1).double()
-        if d.x_ld < d.Cin:                                             # row-packed input: channels run on into the next pixels
-            assert d.KW == 1 and d.pad == 0 and d.groups == 1
-            px = d.Cin // d.x_ld                                       # pixels per K slab
-            raw = xview(d.x_ld).permute(0, 3, 1, 2)
-            wt2 = wt.reshape(d.Cout, px, d.x_ld, d.KH).permute(0, 2, 3, 1)                  # (Cout, c, kh, kw)
-            out = F.conv2d(raw, wt2, stride=d.stride)[..., :d.OH, :d.OW]
-        else:
-            out = F.conv2d(xin, wt, stride=d.stride, padding=d.pad, dilation=d.dil, groups=d.groups)
-        assert out.shape[2] >= d.OH and out.shape[3] >= d.OW, (tuple(out.shape), d.OH, d.OW)
-        out = out[..., :d.OH, :d.OW].permute(0, 2, 3, 1)               # (N, OH, OW, Cout)
-        if bias:
-            if d.bias_n_mod:
-                tab = bias.flat()[:d.bias_n_mod * d.Cout].view(d.bias_n_mod, d.Cout).double()
-                out = out + tab[torch.arange(d.N) % d.bias_n_mod][:, None, None, :]
-            else:
-                out = out + bias.flat()[:d.Cout].double()
-        def resview(p32, psplit, plane, N_, H_, W_, ld_, coff_):
-            if p32:
-                return _pix_view(p32, N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
-            hi = _pix_view(psplit, N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
-            lo = _pix_view(Ptr(psplit.t, psplit.off + plane), N_, H_, W_, ld_, C=d.Cout + coff_)[..., coff_:].double()
-            return hi + lo / 2048.0
-        rs_, rp_ = (f16s.res_split, f16s.res_plane) if f16s is not None else (NULL, 0)
-        r2s_, r2p_ = (f16s.res2_split, f16s.res2_plane) if f16s is not None else (NULL, 0)
-        if d.res_mode == 1:
-            out = out + resview(res, rs_, rp_, d.N, d.OH, d.OW, d.res_ld, d.res_coff)
-        elif d.res_mode == 2:                                          # nearest-upsampled residual (PAFPN top-down)
-            r = resview(res, rs_, rp_, d.N, d.res_H, d.res_W, d.res_ld, d.res_coff)
-            ih = (torch.arange(d.OH) * d.res_H) // d.OH
-            iw = (torch.arange(d.OW) * d.res_W) // d.OW
-            out = out + r[:, ih][:, :, iw]
-        if res2 or r2s_:
-            out = out + resview(res2, r2s_, r2p_, d.N, d.OH, d.OW, d.res2_ld, d.res2_coff)
-        out = _act(out, d.act).float()
-        if y:
-            yv = _pix_view(y, d.N, d.yH, d.yW, d.y_ld, d.y_nstride, 0, d.Cout + d.y_coff)[..., d.y_coff:]
-            yv[:, d.oy_add::d.oy_mul, d.ox_add::d.ox_mul][:, :d.OH, :d.OW] = out
-        if f16s is not None and f16s.y_split:
-            hi, lo = _split_f16(out)
-            for plane, val in ((0, hi), (f16s.y_plane, lo)):
-                pv = Ptr(f16s.y_split.t, f16s.y_split.off + plane)
-                yv = _pix_view(pv, d.N, d.yH, d.yW, d.y_ld, d.y_nstride, 0, d.Cout + d.y_coff)[..., d.y_coff:]
-                yv[:, d.oy_add::d.oy_mul, d.ox_add::d.ox_mul][:, :d.OH, :d.OW] = val
+        out, _ = conv_ref(d, x, w, bias, res, res2, f16s, kmajor_w)
+        conv_store(d, y, f16s.y_split if f16s is not None else NULL, f16s.y_plane if f16s is not None else 0, out.float())
         return 0
 
     def tt_conv2d_f16s(self, d, io, stream):
@@ -501,7 +525,7 @@ class Emu:
     def tt_global_avgpool(self, x, x_ld, x_coff, y, N, HW, Cc, stream):
         self.launches += 1
         v = torch.as_strided(x.flat()[x_coff:], (N, HW, Cc), (HW * x_ld, x_ld, 1))
-        y.flat()[:N * Cc].view(N, Cc).copy_(v.double().mean(1).float())
+        y.flat()[:N * Cc].view(N, Cc).copy_(v.double().mean(1))
         return 0
 
     def tt_broadcast_rows(self, v, y, N, HW, Cc, y_ld, y_coff, stream):
@@ -518,7 +542,7 @@ class Emu:
     def tt_se_pool(self, x, s, N, HW, Cc, stream):
         self.launches += 1
         xv = x.flat()[:N * HW * Cc].view(N, HW, Cc)
-        s.flat()[:N * Cc].view(N, Cc).copy_(0.5 * xv.double().mean(1).float() + 0.5 * xv.amax(1))
+        s.flat()[:N * Cc].view(N, Cc).copy_(0.5 * xv.double().mean(1) + 0.5 * xv.amax(1).double())
         return 0
 
     def tt_se_apply(self, x, g, sc, sc_ld, sc_coff, y, y_ld, y_coff, N, HW, Cc, stream):
@@ -534,7 +558,7 @@ class Emu:
             assert dst.t.dtype == torch.float16 and src.off % 2 == 0 and dst.off % 2 == 0
             src = Ptr(src.t.reshape(-1).view(torch.float32), src.off // 2)
             dst = Ptr(dst.t.reshape(-1).view(torch.float32), dst.off // 2)
-        r = (torch.arange(rows) // rdiv) % rmod
+        r = (torch.arange(rows, device=dst.t.device) // rdiv) % rmod
         n_src = int(r.max()) + 1
         sv = torch.as_strided(src.flat(), (n_src, cols), (src_ld, 1))
         torch.as_strided(dst.flat(), (rows, cols), (dst_ld, 1)).copy_(sv[r])
@@ -545,7 +569,7 @@ class Emu:
         n = rows if not row_count else min(rows, int(row_count.flat()[0]))
         xv = torch.as_strided(x.flat(), (rows, D), (x_ld, 1))[:n].double()
         o = F.layer_norm(xv, (D,), gamma.flat()[:D].double(), beta.flat()[:D].double(), 1e-5)
-        torch.as_strided(y.flat(), (rows, D), (y_ld, 1))[:n] = o.float()
+        torch.as_strided(y.flat(), (rows, D), (y_ld, 1))[:n] = o
         return 0
 
     def tt_eltwise(self, op, act, a, a_ld, b, b_ld, c, c_ld, y, y_ld, rows, cols, stream):
@@ -559,9 +583,11 @@ class Emu:
             o = (1 - A) * v(b, b_ld)
         elif op == 2:
             o = (1 - A) * v(b, b_ld) + A * v(c, c_ld)
+        elif op == 4:                                                  # inverse softplus (a > 0)
+            o = A + torch.log(-torch.expm1(-A))
         else:
-            o = _act(A, act)
-        v(y, y_ld).copy_(o)
+            o = A
+        v(y, y_ld).copy_(_act(o, act))
         return 0
 
     def tt_gru_input(self, wp, ctrl_sp, t, T, buf, ld, B, HW, stream):
@@ -702,10 +728,12 @@ class Emu:
         o = off.flat()[:BN * cap * Hh * L * P * 2].view(BN, cap, Hh, L, P, 2)
         lg = logits.flat()[:BN * cap * Hh * L * P].view(BN, cap, Hh, L * P)
         r = ref.flat()[:BN * cap * 2].view(BN, cap, 1, 1, 1, 2)
-        norm = torch.tensor([[w, h] for h, w in shapes], dtype=torch.float32)
+        norm = torch.tensor([[w, h] for h, w in shapes], dtype=torch.float32, device=o.device)
         loc = r + o / norm[None, None, None, :, None, :]
         aw = lg.softmax(-1).view(BN, cap, Hh, L, P)
-        out.flat()[:BN * cap * Hh * dh].view(BN, cap, Hh * dh).copy_(msda_pytorch(v, torch.tensor(shapes), loc, aw))
+        res = msda_pytorch(v, torch.tensor(shapes), loc, aw)
+        n = min(cap, int(max_len.flat()[0])) if max_len else cap     # rows at or past *max_len are not written
+        out.flat()[:BN * cap * Hh * dh].view(BN, cap, Hh * dh)[:, :n] = res[:, :n]
         return 0
 
     def tt_look_reduce(self, rows, B, cams, cap, Cc, max_len, out, stream):
