@@ -12,7 +12,8 @@ Per call the harness synchronises, snapshots, runs the entry, synchronises again
 Entries that have full-shape checkers of their own are listed in COVERED_ELSEWHERE and only counted; an entry that is in neither map is
 reported, so a new kernel cannot slip in unchecked.
 
-On the GPU the synchronisation serialises the side streams; that changes timing, not results (CUDA graphs stay off).
+On the GPU the synchronisation serialises the side streams; that changes timing, not results (CUDA graphs stay off): every access across
+streams is ordered by an event (the audit of tests/test_stream_order_gpu.py), and adversarial schedules match the serial forward.
 """
 import ctypes as C
 import inspect
