@@ -438,6 +438,34 @@ typedef struct {
 size_t tt_loss_workspace_bytes(int n_terms);
 int tt_loss_reduce(const tt_loss_term* terms, int n_terms, float* out, int n_slots, void* ws, size_t ws_bytes, tt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (11) the camera branch's supervision of the key frame (encoder_decoder_framework.py:171-190, 442-491; utils.py:31-47):
+ *   seg_loss   = weight * FocalLoss(alpha, gamma, ignore_index)(seg logits, nearest-resized labels .long()), the focal transform applied
+ *                to the MEAN cross entropy over the non-ignored pixels (NaN when every pixel is ignored, as torch);
+ *   depth_loss = sum over the foreground cells of BCE-with-logits(depth logits, one-hot bin) / max(1, foreground cells), the bins from
+ *                the min over each factor x factor block of the depth map (0 -> 1e5 first, a NaN pixel makes the block NaN).
+ * Either half is off when its logits pointer is NULL.  Logits are read in place from channels-last maps (class c of pixel p at
+ * logits[p * ld + coff + c]; channels past `classes` / `bins` are never read); the ground truth is the full-resolution fp32 maps.
+ */
+typedef struct {
+  const float* seg_logits;      /* (BN, seg_h, seg_w) pixels of seg_ld floats; NULL: no seg_loss */
+  const float* seg_gt;          /* (BN, seg_H, seg_W) labels as floats; pixel (y, x) reads label (src(y), src(x)), ATen's nearest index */
+  const float* depth_logits;    /* (BN, depth_h, depth_w) pixels of depth_ld floats; NULL: no depth_loss */
+  const float* depth_gt;        /* (BN, depth_h * depth_factor, depth_w * depth_factor) depths */
+  int BN;
+  int seg_h, seg_w, seg_H, seg_W, seg_ld, seg_coff, seg_classes, seg_ignore;
+  float seg_alpha, seg_gamma, seg_weight;
+  int depth_h, depth_w, depth_factor, depth_ld, depth_coff, depth_bins;
+  float depth_offset;           /* fp32 (d_bound[0] - d_bound[2]): bin value v = (min depth - depth_offset) / depth_step in fp32 */
+  float depth_step;             /* fp32 d_bound[2] */
+} tt_camera_loss_desc;
+/* out[0] = seg_loss, out[1] = depth_loss (fp32; a half that is off leaves its slot untouched).  Per-CTA fp64 sums and integer counts,
+ * folded in a fixed order by the last CTA: two calls on the same inputs give bitwise equal results.  A label whose truncation lies
+ * outside [0, seg_classes) and is not seg_ignore (torch raises) makes seg_loss NaN.  ws: tt_camera_loss_workspace_bytes(d) bytes of
+ * device memory, not shared with a concurrent call. */
+size_t tt_camera_loss_workspace_bytes(const tt_camera_loss_desc* d);
+int tt_camera_loss(const tt_camera_loss_desc* d, float* out, void* ws, size_t ws_bytes, tt_stream_t stream);
+
 #ifdef __cplusplus
 }
 /* C++ linkage, mangled exactly like the reference's own definition (ops/voxel_pooling/src/voxel_pooling_forward_cuda.cu:38,

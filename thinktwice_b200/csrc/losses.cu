@@ -108,9 +108,180 @@ __global__ void __launch_bounds__(LOSS_TPB) loss_reduce_kernel(const tt_loss_ter
   if (threadIdx.x == 0) *counter = 0u;
 }
 
+// ---------------------------------------------------------------------------------------------- the camera branch's supervision
+// encoder_decoder_framework.py:171-190, 442-491, utils.py:31-47.  CTAs [0, gs) take pixels of the segmentation map (one thread per pixel),
+// CTAs [gs, gs + gd) take cells of the depth map (one warp per cell: the 16x16 min-pool, then the D logits).  Each CTA writes fp64 sums
+// and integer counts; the last CTA to arrive folds them in CTA order and applies the non-linear finish.
+constexpr int CAM_TPB = 256;
+constexpr int CAM_WARPS = CAM_TPB / 32;
+constexpr int CAM_CTAS_PER_SM = 8;
+
+struct CamPartial {
+  double seg, bce;                      // sum of the cross entropies / of the BCE terms
+  long long nseg, nfg, bad;             // non-ignored pixels / foreground cells / labels torch rejects
+};
+
+// ATen's nearest source index (UpSample.h nearest_idx) for an output of `out` pixels over an input of `in`, scale (float)in / out
+__device__ __forceinline__ long long nearest_src(long long k, int in, int out) {
+  if (out == in) return k;
+  if (out == 2 * in) return k >> 1;
+  const long long s = (long long)floorf(__fmul_rn((float)k, (float)in / (float)out));
+  return s < in - 1 ? s : in - 1;
+}
+
+__device__ __forceinline__ float nan_min(float a, float b) { return (isnan(a) || isnan(b)) ? CUDART_NAN_F : fminf(a, b); }   // torch.min
+
+// log(1 + exp(-|x|)) + max(x, 0) - x * y: BCE with logits for a 0 / 1 target, overflow-free
+__device__ __forceinline__ double bce_logit(double x, bool y) { return fmax(x, 0.0) - (y ? x : 0.0) + log1p(exp(-fabs(x))); }
+
+__device__ void seg_pixels(const tt_camera_loss_desc& d, int cta, int n_ctas, CamPartial& p) {
+  const long long hw = (long long)d.seg_h * d.seg_w, n = (long long)d.BN * hw;
+  for (long long i = (long long)cta * CAM_TPB + threadIdx.x; i < n; i += (long long)n_ctas * CAM_TPB) {
+    const long long bn = i / hw, r = i - bn * hw, y = r / d.seg_w, x = r - y * d.seg_w;
+    const float lab = __ldg(&d.seg_gt[(bn * d.seg_H + nearest_src(y, d.seg_H, d.seg_h)) * d.seg_W + nearest_src(x, d.seg_W, d.seg_w)]);
+    if (!(fabsf(lab) < 2147483648.f)) { ++p.bad; continue; }      // NaN / inf / no int: torch's .long() gives garbage, its CE raises
+    const int l = (int)lab;                                        // .long() truncates toward zero
+    if (l == d.seg_ignore) continue;
+    if (l < 0 || l >= d.seg_classes) { ++p.bad; continue; }
+    const float* q = d.seg_logits + i * d.seg_ld + d.seg_coff;
+    float m = __ldg(q);
+    for (int c = 1; c < d.seg_classes; ++c) m = fmaxf(m, __ldg(q + c));   // a NaN logit still reaches the sum below
+    double s = 0.0;
+    for (int c = 0; c < d.seg_classes; ++c) s += exp((double)__ldg(q + c) - (double)m);
+    p.seg += (double)m + log(s) - (double)__ldg(q + l);
+    ++p.nseg;
+  }
+}
+
+__device__ void depth_cells(const tt_camera_loss_desc& d, int cta, int n_ctas, CamPartial& p) {
+  const int lane = threadIdx.x & 31, f = d.depth_factor, ff = f * f;
+  const long long hw = (long long)d.depth_h * d.depth_w, n = (long long)d.BN * hw;
+  const long long W = (long long)d.depth_w * f, H = (long long)d.depth_h * f;
+  const float top = (float)(d.depth_bins + 1);
+  for (long long i = (long long)cta * CAM_WARPS + (threadIdx.x >> 5); i < n; i += (long long)n_ctas * CAM_WARPS) {
+    const long long bn = i / hw, r = i - bn * hw, cy = r / d.depth_w, cx = r - cy * d.depth_w;
+    const float* g = d.depth_gt + (bn * H + cy * f) * W + cx * f;
+    float mn = CUDART_INF_F;
+    for (int k = lane; k < ff; k += 32) {
+      float v = __ldg(&g[(long long)(k / f) * W + k % f]);
+      mn = nan_min(mn, v == 0.f ? 1e5f : v);
+    }
+    for (int o = 16; o > 0; o >>= 1) mn = nan_min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    const float v = __fdiv_rn(__fsub_rn(mn, d.depth_offset), d.depth_step);
+    const int bin = (v >= 0.f && v < top) ? (int)v : 0;           // NaN / out of range -> class 0, dropped with the one-hot's column 0
+    if (bin < 1) continue;
+    const float* q = d.depth_logits + i * d.depth_ld + d.depth_coff;
+    for (int c = lane; c < d.depth_bins; c += 32) p.bce += bce_logit((double)__ldg(q + c), c == bin - 1);
+    if (lane == 0) ++p.nfg;
+  }
+}
+
+template <typename T>
+__device__ T block_sum(T v, T* red) {                             // fixed shared-memory tree: the same order on every call
+  red[threadIdx.x] = v;
+  __syncthreads();
+  for (int w = CAM_TPB / 2; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  const T s = red[0];
+  __syncthreads();
+  return s;
+}
+
+__device__ CamPartial block_fold(CamPartial p, double* rd, long long* rl) {
+  CamPartial s;
+  s.seg = block_sum(p.seg, rd);
+  s.bce = block_sum(p.bce, rd);
+  s.nseg = block_sum(p.nseg, rl);
+  s.nfg = block_sum(p.nfg, rl);
+  s.bad = block_sum(p.bad, rl);
+  return s;
+}
+
+__global__ void __launch_bounds__(CAM_TPB) camera_loss_kernel(const tt_camera_loss_desc d, int gs, int gd, CamPartial* __restrict__ part,
+                                                              unsigned* counter, float* __restrict__ out) {
+  __shared__ double rd[CAM_TPB];
+  __shared__ long long rl[CAM_TPB];
+  __shared__ bool last;
+  CamPartial p{0.0, 0.0, 0, 0, 0};
+  if ((int)blockIdx.x < gs) seg_pixels(d, blockIdx.x, gs, p);
+  else depth_cells(d, blockIdx.x - gs, gd, p);
+  const CamPartial s = block_fold(p, rd, rl);
+  if (threadIdx.x == 0) {
+    part[blockIdx.x] = s;
+    __threadfence();
+    last = atomicAdd(counter, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  CamPartial a{0.0, 0.0, 0, 0, 0};
+  for (int b = threadIdx.x; b < (int)gridDim.x; b += CAM_TPB) {
+    const CamPartial* q = &part[b];
+    a.seg += __ldcg(&q->seg); a.bce += __ldcg(&q->bce);
+    a.nseg += __ldcg(&q->nseg); a.nfg += __ldcg(&q->nfg); a.bad += __ldcg(&q->bad);
+  }
+  const CamPartial t = block_fold(a, rd, rl);
+  if (threadIdx.x == 0) {
+    if (gs > 0) {
+      const double ce = t.bad ? CUDART_NAN : t.seg / (double)t.nseg;              // no pixel left: 0 / 0 = NaN, as torch's mean
+      const double logpt = -ce;                                                     // utils.py:43-46, on the batch-mean CE
+      out[0] = (float)(-pow(1.0 - exp(logpt), (double)d.seg_gamma) * (double)d.seg_alpha * logpt * (double)d.seg_weight);
+    }
+    if (gd > 0) out[1] = (float)(t.bce / (double)(t.nfg > 0 ? t.nfg : 1));
+    *counter = 0u;
+  }
+}
+
+// CTAs of each half: enough for the work, the SMs' worth shared out by the bytes each half reads per unit of work
+void camera_grid(const tt_camera_loss_desc& d, int& gs, int& gd) {
+  const long long ns = d.seg_logits ? (long long)d.BN * d.seg_h * d.seg_w : 0;
+  const long long nd = d.depth_logits ? (long long)d.BN * d.depth_h * d.depth_w : 0;
+  const double bs = (double)ns * (d.seg_classes + 1), bd = (double)nd * ((double)d.depth_factor * d.depth_factor + d.depth_bins);
+  const int budget = tt_num_sms() * CAM_CTAS_PER_SM;
+  const long long want_s = (ns + CAM_TPB - 1) / CAM_TPB, want_d = (nd + CAM_WARPS - 1) / CAM_WARPS;
+  long long cap_s = bs + bd > 0 ? (long long)(budget * bs / (bs + bd)) : 0;
+  if (ns && cap_s < 1) cap_s = 1;
+  long long cap_d = budget - cap_s;
+  if (nd && cap_d < 1) cap_d = 1;
+  gs = (int)(want_s < cap_s ? want_s : cap_s);
+  gd = (int)(want_d < cap_d ? want_d : cap_d);
+}
+
 }  // namespace
 
 extern "C" {
+
+size_t tt_camera_loss_workspace_bytes(const tt_camera_loss_desc* d) {
+  int gs = 0, gd = 0;
+  if (d) camera_grid(*d, gs, gd);
+  return (size_t)(gs + gd) * sizeof(CamPartial) + 256;
+}
+
+int tt_camera_loss(const tt_camera_loss_desc* d, float* out, void* ws, size_t ws_bytes, tt_stream_t stream) {
+  TT_REQUIRE(d && out && ws && d->BN > 0 && (d->seg_logits || d->depth_logits), "tt_camera_loss", "bad arguments");
+  TT_REQUIRE(!d->seg_logits || (d->seg_gt && d->seg_h > 0 && d->seg_w > 0 && d->seg_H > 0 && d->seg_W > 0 && d->seg_classes > 0 &&
+                                d->seg_coff >= 0 && d->seg_coff + d->seg_classes <= d->seg_ld),
+             "tt_camera_loss", "bad segmentation half");
+  TT_REQUIRE(!d->depth_logits || (d->depth_gt && d->depth_h > 0 && d->depth_w > 0 && d->depth_factor > 0 && d->depth_bins > 0 &&
+                                  d->depth_coff >= 0 && d->depth_coff + d->depth_bins <= d->depth_ld && d->depth_step > 0.f),
+             "tt_camera_loss", "bad depth half");
+  TT_REQUIRE(ws_bytes >= tt_camera_loss_workspace_bytes(d), "tt_camera_loss", "workspace too small");
+  int gs, gd;
+  camera_grid(*d, gs, gd);
+  cudaStream_t s = (cudaStream_t)stream;
+  CamPartial* part = (CamPartial*)ws;
+  unsigned* counter = (unsigned*)((char*)ws + (size_t)(gs + gd) * sizeof(CamPartial));
+  if (cudaMemsetAsync(counter, 0, sizeof(unsigned), s) != cudaSuccess) {
+    tt_set_error("tt_camera_loss: clearing the arrival counter failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return TT_ERR_CUDA;
+  }
+  camera_loss_kernel<<<gs + gd, CAM_TPB, 0, s>>>(*d, gs, gd, part, counter, out);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH("tt_camera_loss");
+  return TT_OK;
+}
 
 size_t tt_loss_workspace_bytes(int n_terms) {
   return terms_bytes(n_terms) + (size_t)n_terms * LOSS_CHUNKS * sizeof(double) + 256;

@@ -5,6 +5,7 @@ same registry name, same constructor keywords, same `forward_inference(batch)` /
 `control_pid` signatures and the same pred dict, so `leaderboard/team_code/thinktwice_agent.py:456-461`
 calls it unchanged.  The forward runs entirely in libtt_b200 (no eager / CPU fallback).
 """
+import ctypes
 import time
 from collections import OrderedDict, deque
 
@@ -63,6 +64,8 @@ class EncoderDecoder(nn.Module):
         super().__init__()
         self.config = train_cfg
         self.num_cams = num_cams
+        self.downsample_factor = downsample_factor                # depth supervision: min-pool block of the depth ground truth
+        self.seg_downsample_factor = seg_downsample_factor        # segmentation supervision: nearest resize of the labels
         self.model_cfg = dict(img_encoder=img_encoder, decoder=decoder, lidar_encoder=lidar_encoder)
         self.turn_controller = PIDController(K_P=train_cfg['turn_KP'], K_I=train_cfg['turn_KI'], K_D=train_cfg['turn_KD'], n=train_cfg['turn_n'])
         self.speed_controller = PIDController(K_P=train_cfg['speed_KP'], K_I=train_cfg['speed_KI'], K_D=train_cfg['speed_KD'], n=train_cfg['speed_n'])
@@ -526,15 +529,15 @@ class EncoderDecoder(nn.Module):
 
     @torch.no_grad()
     def forward_train(self, batch):
-        """framework:147-191: the network over both sweeps, the decoder with teacher forcing, ThinkTwiceDecoder.loss.  The camera
-        branch's depth / segmentation supervision (train_cfg use_depth / use_seg) is not built: such a model raises.  Runs eagerly on
-        the inference arena without touching its CUDA graphs; a validation batch is not the next closed-loop tick, so the streaming
-        BEV cache starts over afterwards."""
-        cfg = self.config
-        missing = [n for n, k in (('depth_loss', 'use_depth'), ('seg_loss', 'use_seg')) if k in cfg and cfg[k]]
+        """framework:147-191: the network over both sweeps, the decoder with teacher forcing, ThinkTwiceDecoder.loss, then the camera
+        branch's supervision of the key frame when train_cfg turns it on: seg_loss (use_seg, ground truth batch['seg']) and depth_loss
+        (use_depth, batch['depth']), one tt_camera_loss launch.  A flag whose ground truth is absent raises NotImplementedError.  Runs
+        eagerly on the inference arena without touching its CUDA graphs; a validation batch is not the next closed-loop tick, so the
+        streaming BEV cache starts over afterwards."""
+        terms = self._camera_terms()
+        missing = [f"{name} (train_cfg {flag}) needs batch['{key}']" for name, flag, key in terms if key not in batch]
         if missing:
-            raise NotImplementedError(f'{" and ".join(missing)} (train_cfg use_depth / use_seg) are not built yet: set them False to '
-                                      'evaluate the decoder losses')
+            raise NotImplementedError('; '.join(missing) + ': pass the ground truth, or set the flag False to evaluate the other losses')
         if self.eng is None:
             im0 = self._batch_images(batch)
             self.prepare(im0.device if im0.is_cuda else 'cuda:0')
@@ -555,11 +558,83 @@ class EncoderDecoder(nn.Module):
         flat, bev32, mid, lidar_hi = self.get_fusion_feat(cam['bev'], lidar[0])
         teacher = {k: batch[k] for k in ('waypoints', 'action_sigma', 'action_mu', 'future_action_sigma', 'future_action_mu')}
         pred = self.decoder(flat, bev32, meas, None, self, teacher, [None, None, cam['fpn_feats'], lidar_hi])
+        self._check_camera_gt(batch, cam, B_now, terms)           # before any ground truth is staged
         losses = self.decoder.loss(batch, pred, mid)
+        losses.update(self.camera_loss(batch, cam, terms))
         self.img_encoder.reset_stream()
         self.last_cam_feat = cam
         self.last_train = dict(pred=pred, mid=mid, flat=flat, bev32=bev32, meas=meas, lidar_hi=lidar_hi)   # for parity checks
         return losses
+
+    # ------------------------------------------------------------------ camera supervision (framework:171-190, 442-491; utils.py:31-47)
+    CAMERA_TERMS = (('seg_loss', 'use_seg', 'seg'), ('depth_loss', 'use_depth', 'depth'))     # the reference's key order
+    SEG_IGNORE, SEG_ALPHA, SEG_GAMMA, SEG_WEIGHT = 255, 0.5, 2.0, 10.0                          # FocalLoss() defaults; seg_loss * 10
+
+    def _camera_terms(self):
+        cfg = self.config
+        return [t for t in self.CAMERA_TERMS if t[1] in cfg and cfg[t[1]]]
+
+    def _check_camera_gt(self, batch, cam, B, terms):
+        """the key frame's depth / segmentation ground truth against the maps it supervises; ValueError where the reference fails (a view
+        or shape error, or CrossEntropyLoss's target-out-of-bounds error).  Depth values are not checked: every value has a result."""
+        for _, _, key in terms:
+            fm, gt = cam[key], batch[key]
+            N = fm.N // B
+            if key == 'depth':
+                f = self.downsample_factor
+                want = (B, N, f * fm.H, f * fm.W)
+                if tuple(gt.shape) != want:
+                    raise ValueError(f'depth: expected shape {want} (the {fm.H}x{fm.W} depth map, {f}x{f} blocks), got {tuple(gt.shape)}')
+                continue
+            s = self.seg_downsample_factor
+            if gt.dim() != 4 or tuple(gt.shape[:2]) != (B, N) or gt.shape[2] // s != fm.H or gt.shape[3] // s != fm.W:
+                raise ValueError(f'seg: expected (B, N, H, W) = ({B}, {N}, H, W) with H // {s} = {fm.H} and W // {s} = {fm.W}, got '
+                                 f'{tuple(gt.shape)}')
+            # the labels the loss reads: T.Resize(NEAREST) (= F.interpolate 'nearest') of the full-resolution map, then .long()
+            lab = torch.nn.functional.interpolate(gt.reshape(B * N, 1, *gt.shape[2:]).float(), size=(fm.H, fm.W), mode='nearest')
+            if not bool(torch.isfinite(lab).all()):
+                raise ValueError('seg: a label the loss reads is not finite')
+            t = lab.trunc()
+            if not bool((((t >= 0) & (t < fm.C)) | (t == self.SEG_IGNORE)).all()):
+                raise ValueError(f'seg: labels must truncate into [0, {fm.C}) or to {self.SEG_IGNORE} (ignored)')
+
+    def camera_loss(self, batch, cam, terms):
+        """seg_loss / depth_loss of the key frame (cam = key_device's maps, before the next forward overwrites them), from ONE
+        tt_camera_loss launch reading the logits in place: an OrderedDict of fresh 0-d fp32 device tensors in the reference's order."""
+        if not terms:
+            return OrderedDict()
+        vals = self.launch_camera_loss(self.stage_camera_supervision(batch, cam, terms))
+        return OrderedDict((name, vals[0 if key == 'seg' else 1]) for name, _, key in terms)
+
+    def stage_camera_supervision(self, batch, cam, terms):
+        """host half of camera_loss: the ground truth staged by name (gt.seg, gt.depth) from host or device memory (_check_camera_gt has
+        vetted it), and the tt_camera_loss descriptor over it and the logit maps."""
+        e = self.eng
+        keys = [k for _, _, k in terms]
+        BN = cam[keys[0]].N
+        f = dict(BN=BN, seg_logits=lib._p(None), seg_gt=lib._p(None), depth_logits=lib._p(None), depth_gt=lib._p(None))
+        if 'seg' in keys:
+            fm, gt = cam['seg'], batch['seg']
+            H, W = gt.shape[2:]
+            g = e.upload('gt.seg', gt.float().reshape(BN, H, W).contiguous())
+            f.update(seg_logits=lib._p(fm.t), seg_gt=lib._p(g), seg_h=fm.H, seg_w=fm.W, seg_H=H, seg_W=W, seg_ld=fm.ld, seg_coff=fm.coff,
+                     seg_classes=fm.C, seg_ignore=self.SEG_IGNORE, seg_alpha=self.SEG_ALPHA, seg_gamma=self.SEG_GAMMA,
+                     seg_weight=self.SEG_WEIGHT)
+        if 'depth' in keys:
+            fm, gt = cam['depth'], batch['depth']
+            d0, _, step = (float(v) for v in self.dbound)
+            g = e.upload('gt.depth', gt.float().reshape(BN, *gt.shape[2:]).contiguous())
+            f.update(depth_logits=lib._p(fm.t), depth_gt=lib._p(g), depth_h=fm.H, depth_w=fm.W, depth_factor=self.downsample_factor,
+                     depth_ld=fm.ld, depth_coff=fm.coff, depth_bins=self.img_encoder.depth_channels, depth_offset=d0 - step, depth_step=step)
+        return lib.camera_loss_desc(**f)
+
+    def launch_camera_loss(self, d):
+        """one tt_camera_loss launch on the current stream: a fresh (2,) fp32 tensor [seg_loss, depth_loss]."""
+        e = self.eng
+        out = e.buf('loss.cam', (2,))
+        ws = e.buf('loss.cam_ws', (int(lib.load().tt_camera_loss_workspace_bytes(lib.ref(d))),), torch.uint8)
+        lib.call('tt_camera_loss', lib.ref(d), lib._p(out), lib._p(ws), ctypes.c_size_t(ws.numel()))
+        return out.clone()                                         # the caller owns its losses (the arena buffer is reused)
 
     @staticmethod
     def _parse_losses(losses):

@@ -89,6 +89,15 @@ class LossTerm(C.Structure):
                 ('ndim', C.c_int), ('kind', C.c_int), ('slot', C.c_int), ('aux', C.c_int), ('scale', C.c_double)]
 
 
+class CameraLossDesc(C.Structure):
+    """tt_camera_loss_desc (include/tt_b200.h section 11): the segmentation and depth halves of tt_camera_loss."""
+    _fields_ = [('seg_logits', C.c_void_p), ('seg_gt', C.c_void_p), ('depth_logits', C.c_void_p), ('depth_gt', C.c_void_p), ('BN', C.c_int)] + \
+               [(n, C.c_int) for n in ('seg_h', 'seg_w', 'seg_H', 'seg_W', 'seg_ld', 'seg_coff', 'seg_classes', 'seg_ignore')] + \
+               [(n, C.c_float) for n in ('seg_alpha', 'seg_gamma', 'seg_weight')] + \
+               [(n, C.c_int) for n in ('depth_h', 'depth_w', 'depth_factor', 'depth_ld', 'depth_coff', 'depth_bins')] + \
+               [('depth_offset', C.c_float), ('depth_step', C.c_float)]
+
+
 _lib = None
 
 
@@ -104,7 +113,7 @@ def load():
     lib.tt_last_error.restype = C.c_char_p
     lib.tt_launch_count.restype = C.c_longlong
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
-              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes'):
+              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -120,7 +129,7 @@ EXPORTS = [
     'tt_voxelize_workspace_bytes', 'tt_voxelize_mean', 'tt_rulebook_workspace_bytes', 'tt_sparse_rulebook',
     'tt_sparse_conv', 'tt_sparse_to_bev', 'tt_conv2d_f16s', 'tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_pointwise_f16s', 'tt_upsample2x_bilinear_ac_split', 'tt_f16s_saturation_count', 'tt_sparse_conv_f16s', 'tt_sparse_conv_os_f16s', 'tt_look_project', 'tt_look_rebatch', 'tt_msda_forward', 'tt_look_reduce', 'tt_msda_forward_frames', 'tt_look_reduce_frames', 'tt_gru_input',
     'tt_preprocess_u8', 'tt_lidar_stitch', 'tt_points_union', 'tt_voxel_pooling_backward', 'tt_ms_deform_attn_forward', 'tt_ms_deform_attn_backward',
-    'tt_loss_workspace_bytes', 'tt_loss_reduce',
+    'tt_loss_workspace_bytes', 'tt_loss_reduce', 'tt_camera_loss_workspace_bytes', 'tt_camera_loss',
 ]
 
 
@@ -135,6 +144,14 @@ def pack_loss_terms(terms):
         for d, (n, ps, gs) in enumerate(zip(t['shape'], t['pred_stride'], t['gt_stride'])):
             a.shape[d], a.pred_stride[d], a.gt_stride[d] = n, ps, gs
     return arr
+
+
+def camera_loss_desc(**fields):
+    """CameraLossDesc's field names (pointers from `_p`; an absent half's pointers NULL) -> the descriptor tt_camera_loss reads."""
+    d = CameraLossDesc()
+    for k, v in fields.items():
+        setattr(d, k, v)
+    return d
 
 
 def _stream():

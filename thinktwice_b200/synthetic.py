@@ -117,3 +117,40 @@ def make_supervision(cfg, batch_size=1, seed=0, device='cpu'):
                 future_action_mu=list(st('future_action_mu').unbind(1)), future_action_sigma=list(st('future_action_sigma').unbind(1)),
                 value=st('value').view(-1), feature=st('feature'), grid_feature=grid,
                 future_grid_feature=[[None, None, fut[:, t]] for t in range(T)])
+
+
+def make_camera_supervision(cfg, batch_size=1, seed=0, device='cpu'):
+    """Seeded ground truth of the camera branch's supervision (encoder_decoder_framework.py:171-190): depth and seg, (B, N, H, W) fp32 at the
+    image size.  Depth: dense over the d_bound range and beyond, about 30 % zero pixels (no measurement), in camera 0 one all-zero block,
+    one block holding a NaN, and blocks whose minimum lies exactly on the bin value v = (d - (d_bound[0] - d_bound[2])) / d_bound[2]
+    = 0, 1, 2, D, D + 1 or just below 1 and D + 1.  Seg: labels of the C classes as the data pipeline's grid-sample leaves them, with
+    fractional parts (some just below the next integer) and about 10 % ignored pixels (255, some 255.5).  One generator per frame."""
+    tcfg, enc = cfg.model.train_cfg, cfg.model.img_encoder
+    H, W = tcfg['img_size']
+    n = len(CAMERAS)
+    d0, d1, step = (float(v) for v in enc['d_bound'])
+    D = int((d1 - d0) / step)
+    f = int(cfg.model.get('downsample_factor', 16))
+    C = int(enc['seg_net_conf']['out_channels'])
+    edges = [0.0, 1.0, 2.0, float(D), float(D + 1), 1.0 - 2.0 ** -10, D + 1 - 2.0 ** -10]
+    depth, seg = [], []
+    for j in range(batch_size):
+        g = torch.Generator().manual_seed(9000 + 1000 * seed + j)
+        d = (d0 - 2 * step) + (d1 - d0 + 8 * step) * torch.rand(n, H, W, generator=g)
+        d[torch.rand(n, H, W, generator=g) < 0.3] = 0.0
+        d[0, :f, :f] = 0.0                                        # a block with no measurement: background
+        d[0, :f, f:2 * f] = 0.5 * (d0 + d1)
+        d[0, 3, f + 5] = float('nan')                              # torch.min propagates it: background
+        for k, v in enumerate(edges):                              # minimum exactly on a bin value
+            blk = d[0, f:2 * f, k * f:(k + 1) * f]
+            blk.copy_(d1 + 4 * step + torch.rand(f, f, generator=g))
+            blk[int(torch.randint(0, f, (1,), generator=g)), int(torch.randint(0, f, (1,), generator=g))] = (d0 - step) + v * step
+        depth.append(d)
+        lab = torch.randint(0, C, (n, H, W), generator=g).float() + 0.999 * torch.rand(n, H, W, generator=g)
+        below = torch.rand(n, H, W, generator=g) < 0.05
+        lab = torch.where(below, lab.floor() + (1 - 2.0 ** -10), lab)           # just below the next integer: still truncates down
+        ign = torch.rand(n, H, W, generator=g)
+        lab = torch.where(ign < 0.1, torch.full_like(lab, 255.0), lab)
+        lab = torch.where(ign < 0.02, torch.full_like(lab, 255.5), lab)
+        seg.append(lab)
+    return dict(depth=torch.stack(depth).to(device), seg=torch.stack(seg).to(device))

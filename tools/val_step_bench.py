@@ -4,6 +4,10 @@ the same batch, in the same process, the two alternated step by step.  Full thin
 off, device-resident batch.  The card's name, power limit and SM clocks are read in the same call (nvidia-smi queries only).
 
     python tools/val_step_bench.py [--batch 16] [--steps 7]     -> one JSON line (milliseconds: median, min, max over --steps)
+
+--camera-supervision: the config's use_depth / use_seg as shipped (on) and the camera ground truth in the batch.  The validation step
+with seg_loss and depth_loss is then alternated with the same step with the two flags off, and the tt_camera_loss launch is timed alone
+(CUDA events over --launches launches on the staged ground truth), next to the bytes it must read, computed from the shapes.
 """
 import argparse
 import json
@@ -34,13 +38,19 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--batch', type=int, default=16)
     ap.add_argument('--steps', type=int, default=7)
+    ap.add_argument('--camera-supervision', action='store_true')
+    ap.add_argument('--launches', type=int, default=50)
     args = ap.parse_args()
     cfg = Config.fromfile(DEFAULT_CONFIG)
-    for k in ('use_depth', 'use_seg'):
-        cfg.merge_from_dict({f'model.train_cfg.{k}': False})
+    if not args.camera_supervision:
+        for k in ('use_depth', 'use_seg'):
+            cfg.merge_from_dict({f'model.train_cfg.{k}': False})
     m = build_model(cfg.model).prepare('cuda:0')
     batch = make_batch(cfg, args.batch, seed=0, num_points=40000, device='cuda')
     sup = make_supervision(cfg, args.batch, seed=0, device='cuda')
+    if args.camera_supervision:
+        from thinktwice_b200.synthetic import make_camera_supervision
+        sup.update(make_camera_supervision(cfg, args.batch, seed=0, device='cuda'))
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -49,6 +59,14 @@ def main():
         torch.cuda.synchronize()
         return (time.perf_counter() - t0) * 1e3
     runs = {'inference_eager': lambda: m.forward_inference(batch), 'validation_step': lambda: m.forward(is_eval=True, **batch, **sup)}
+    if args.camera_supervision:
+        def without_camera():
+            m.config['use_depth'] = m.config['use_seg'] = False
+            try:
+                m.forward(is_eval=True, **batch, **sup)
+            finally:
+                m.config['use_depth'] = m.config['use_seg'] = True
+        runs['validation_step_no_camera'] = without_camera
     for fn in runs.values():                                         # the first call of each allocates its buffers
         timed(fn)
     ts = {k: [] for k in runs}
@@ -61,7 +79,33 @@ def main():
     out = {k + '_ms': stat(v) for k, v in ts.items()}
     out.update(batch=args.batch, steps=args.steps, gpu=state,
                ratio=round(out['validation_step_ms']['median'] / out['inference_eager_ms']['median'], 3))
+    if args.camera_supervision:
+        out['camera_loss_kernel'] = camera_kernel(m, batch, sup, args.launches)
     print(json.dumps(out))
+
+
+def camera_kernel(m, batch, sup, launches):
+    """tt_camera_loss alone on the ground truth the last step staged: milliseconds per launch (CUDA events around `launches` launches)
+    and the bytes the launch must read (the C logits of each segmentation pixel, its label, each depth block, the D logits of a cell)."""
+    import torch
+    m.forward(is_eval=True, **batch, **sup)
+    terms, cam = m._camera_terms(), m.last_cam_feat
+    d = m.stage_camera_supervision(sup, cam, terms)
+    m.launch_camera_loss(d)
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(launches):
+        m.launch_camera_loss(d)
+    b.record()
+    torch.cuda.synchronize()
+    ms = a.elapsed_time(b) / launches
+    sg, dp = cam['seg'], cam['depth']
+    f, D = m.downsample_factor, m.img_encoder.depth_channels
+    parts = dict(seg_logits=sg.N * sg.H * sg.W * sg.C * 4, seg_labels=sg.N * sg.H * sg.W * 4,
+                 depth_gt=dp.N * dp.H * dp.W * f * f * 4, depth_logits=dp.N * dp.H * dp.W * D * 4)
+    total = sum(parts.values())
+    return dict(ms=round(ms, 4), launches=launches, bytes={k: v for k, v in parts.items()}, total_bytes=total,
+                effective_tb_s=round(total / (ms * 1e-3) / 1e12, 3))
 
 
 if __name__ == '__main__':
