@@ -371,7 +371,8 @@ typedef struct {
  * no antialias: torchvision 0.13.1 of docs/INSTALL.md] -> crop -> /div -> (x - mean) / std.
  * map_grid: fp32 [H][W][2] normalised (x, y) exactly as transform.py:237-240 builds it (one map for every image; may be NULL without
  * undistort).  out_nchw: fp32 [n_img][3][outH][outW] (the `img` tensor of the batch dict) and / or out_split8: the row-packed stem's
- * operand planes [2][n_img][pad_H][pad_W][8 halves] (plane stride split_plane halves; border never written).  Either may be NULL. */
+ * operand planes [2][n_img][pad_H][pad_W][8 halves] (plane stride split_plane halves; border never written).  Either may be NULL.
+ * With out_split8, n_img * pad_H * pad_W * 8 > split_plane (the slots would run past a plane) is refused with TT_ERR_INVALID. */
 int tt_preprocess_u8(const tt_preproc_desc* d, const uint8_t* raw, const float* map_grid, float* out_nchw, void* out_split8,
                      long long split_plane, tt_stream_t stream);
 /* thinktwice_agent.py:340-352: out [n_prev + n_now][4] = [rel_mat (4x4 fp64, row-major, DEVICE) applied to prev's xyz | now], z += z_add (2.5);

@@ -177,13 +177,14 @@ def conv_store(d, y, y_split, y_plane, out):
 class Emu:
     def __init__(self):
         self.launches = 0
+        self.error = b'emulated'
 
     # ------------------------------------------------------------------ bookkeeping
     def tt_version(self):
         return 1
 
     def tt_last_error(self):
-        return b'emulated'
+        return self.error
 
     def tt_launch_count(self):
         return self.launches
@@ -248,9 +249,12 @@ class Emu:
     def tt_preprocess_u8(self, d, raw, map_grid, out_nchw, out_split8, split_plane, stream):
         """include/tt_b200.h section 8: uint8 HWC frames -> grid_sample -> bilinear resize -> crop -> / div -> (x - mean) / std, written as
         fp32 NCHW and / or the stem's split planes (plain torch ops: the semantics, not the kernel's operation order)."""
-        self.launches += 1
         d = _desc(d)
         n, H, W = d.n_img, d.H, d.W
+        if out_split8 and n * d.pad_H * d.pad_W * 8 > _v(split_plane):
+            self.error = b'tt_preprocess_u8: n_img stem slots exceed the stem-plane capacity split_plane'
+            return -1
+        self.launches += 1
         x = raw.flat()[:n * H * W * 3].view(n, H, W, 3).float().permute(0, 3, 1, 2)
         if d.undistort:
             g = map_grid.flat()[:H * W * 2].view(1, H, W, 2).expand(n, H, W, 2)

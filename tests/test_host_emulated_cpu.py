@@ -83,8 +83,12 @@ def test_full_thinktwice_config_through_the_emulated_abi_matches_the_oracle(emul
 def test_raw_uint8_frames_through_the_emulated_abi_match_the_preprocessed_tensor(emulated, impl):
     """SURVEY 8f f1 host plumbing on the CPU: a batch carrying `img_raw` (uint8 frames; per-sweep uint8 staging buffers, the pre-processor
     writing the stem's operand planes — impl 4 — or the NCHW tensor the fp32 engines stage themselves — impl 1) against the same model fed
-    with the oracle's pre-processed `img`."""
+    with the oracle's pre-processed `img`.  Frames of another size than the pre-processor's, and a pre-processor whose final_dim is not
+    the model's, are refused with TTError before anything is pre-processed (the f16s stem slots are sized by the model: a mismatch would
+    leave stale bytes in them, or write past the planes)."""
+    import ctypes as C
     from oracle import preprocess as op
+    from thinktwice_b200 import lib
     from thinktwice_b200.config import PLUMBING_CONFIG
     from thinktwice_b200.preprocess import AgentPreprocessor
     o, m, batch = _pair(PLUMBING_CONFIG, 1, 1200, 7, impl, sweeps=2)
@@ -100,6 +104,28 @@ def test_raw_uint8_frames_through_the_emulated_abi_match_the_preprocessed_tensor
     got = m.forward_inference(rb)
     for k, v in want.items():
         assert rel(got[k], v) < 1e-5, k
+    calls = []
+    emu_pre = emulated.tt_preprocess_u8
+    emulated.tt_preprocess_u8 = lambda *a: calls.append(a) or emu_pre(*a)
+    for h in (200, 400):                                                # fewer bytes than 8 frames / more than the 8 stem slots hold
+        bad = dict(rb, img_raw=torch.from_numpy(np.random.default_rng(h).integers(0, 256, size=(1, 2, 4, h, 400, 3), dtype=np.uint8)))
+        with pytest.raises(lib.TTError, match='raw frames must be uint8'):
+            m.forward_inference(bad)
+        assert not calls, h
+    pre = m.img_encoder.pre
+    with pytest.raises(lib.TTError, match='final_dim'):                 # a 128 x 256 image in a 256 x 256 slot: refused at attach time
+        m.attach_preprocessor(AgentPreprocessor(dict(undistort=True, num_cams=4), dict(conf, final_dim=(128, 256)), 'cpu', map_grid=grid))
+    assert m.img_encoder.pre is pre
+    # the emulated C ABI refuses stem planes one slot short, as the kernel does, and takes them at exactly n slots
+    n, pad = 8, (256 + 6, 256 + 8, 3, 3)
+    slot = pad[0] * pad[1] * 8
+    planes = torch.zeros(2, n * slot, dtype=torch.float16)
+    frames = raw.reshape(n, 300, 400, 3).contiguous()
+    for cap, rc in ((n * slot - slot, -1), (n * slot, 0)):
+        got_rc = emulated.tt_preprocess_u8(C.byref(pre.desc(n, pad)), lib._p(frames), lib._p(pre.grid), lib._p(None), lib._p(planes),
+                                           C.c_longlong(cap), None)
+        assert got_rc == rc, cap
+    assert b'stem-plane capacity' in emulated.tt_last_error()
     with pytest.raises(Exception):                                      # without a pre-processor the raw batch is refused, not guessed at
         m.img_encoder.pre = None
         m.forward_inference(rb)

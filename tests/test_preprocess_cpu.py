@@ -127,6 +127,51 @@ def test_kernel_operation_order_equals_torch_bit_for_bit(undistort):
     assert torch.equal(got, want), float((got - want).abs().max())
 
 
+def test_stem_plane_checker_rejects_each_corruption():
+    """negative controls of tests/stem_plane_checks.py (the full-shape GPU test's judge): planes built here from an independent split
+    (the emulated ABI's) pass; a flipped lo' bit in the last image, one written border pixel, a non-zero pad channel and a write into the
+    guard gap are each rejected, by the property they break."""
+    from emu_lib import _split_f16
+    from stem_plane_checks import sentinel_planes, stem_plane_failures
+    n, H0, W0 = 3, 5, 7
+    pad = (H0 + 3, W0 + 4, 1, 2)
+    slot = pad[0] * pad[1] * 8
+    split_plane = n * slot + 8 * 5
+    v = torch.from_numpy(np.random.default_rng(4).standard_normal((n, 3, H0, W0)).astype(np.float32))
+    v[0, 0, 0, 0], v[1, 2, 4, 6] = 1e5, -3e-9                          # saturating and subnormal-lo values
+    planes = sentinel_planes(split_plane, 'cpu')
+    view = planes.view(2, split_plane)[:, :n * slot].view(2, n, pad[0], pad[1], 8)
+    for p, half in enumerate(_split_f16(v.permute(0, 2, 3, 1))):
+        view[p, :, 1:1 + H0, 2:2 + W0, :3] = half
+        view[p, :, 1:1 + H0, 2:2 + W0, 3:] = 0
+    assert stem_plane_failures(planes, split_plane, v, pad) == []
+
+    def corrupted(edit):
+        bad = planes.clone()
+        edit(bad.view(torch.int16).view(2, split_plane))
+        return stem_plane_failures(bad, split_plane, v, pad)
+
+    def flip_lo(b):
+        b[1, (n - 1) * slot + ((1 + H0 - 1) * pad[1] + 2 + W0 - 1) * 8 + 2] ^= 1      # last image, last interior pixel, channel 2
+    fails = corrupted(flip_lo)
+    assert len(fails) == 1 and fails[0].startswith("lo' plane") and '[2, 4, 6, 2]' in fails[0], fails
+
+    def write_border(b):
+        b[0, slot + (pad[0] - 1) * pad[1] * 8 + 3] = 0                   # image 1, bottom border row, channel 3
+    fails = corrupted(write_border)
+    assert len(fails) == 1 and fails[0].startswith('border pixels'), fails
+
+    def pad_channel(b):
+        b[0, ((1 + 2) * pad[1] + 2 + 3) * 8 + 5] = 0x3C00                # image 0, interior pixel, channel 5 = 1.0
+    fails = corrupted(pad_channel)
+    assert len(fails) == 1 and fails[0].startswith('pad channels'), fails
+
+    def gap(b):
+        b[1, n * slot + 7] = 0
+    fails = corrupted(gap)
+    assert len(fails) == 1 and fails[0].startswith('guard gap'), fails
+
+
 def test_union2one_restatements_match_the_reference_function(golden):
     """carla_dataset.py:250-334 run from its own source text (golden) vs the oracle restatement and vs the product's host half (union_metas)."""
     from make_preprocess_golden import union_case

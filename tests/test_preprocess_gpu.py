@@ -68,6 +68,61 @@ def test_small_frames_edges_and_stem_planes(undistort):
     assert rc == -1 and b'crop' in lib.load().tt_last_error()
 
 
+def agent_frames(n, seed):
+    """n random 900 x 1600 frames, with whole frames and blocks at 0 and 255: frame 0 black, frame n - 1 white, frame 1 with saturated
+    corner blocks on the frame's edges, frame n - 2 a white block holding a black one (sharp 0 / 255 edges inside the crop)."""
+    raw = np.random.default_rng(seed).integers(0, 256, size=(n, 900, 1600, 3), dtype=np.uint8)
+    raw[0], raw[n - 1] = 0, 255
+    raw[1, :300, :500], raw[1, 600:, 1100:] = 0, 255
+    raw[n - 2, 200:700, 400:1200] = 255
+    raw[n - 2, 350:550, 700:900] = 0
+    return torch.from_numpy(raw)
+
+
+@pytest.mark.parametrize('n', [8, 128])
+def test_stem_planes_at_the_agent_shape(n):
+    """the mode the f16s forward uses (`img.nhwc#s8`) at thinktwice.py's geometry — real rectification map, 900 x 1600 -> resize 0.56 ->
+    crop 448 x 896, stem slot 454 x 904 x 8 — for n = 8 images (B = 1 x 2 sweeps x 4 cams) and n = 128 (B = 16).  One call writes both
+    outputs into planes pre-filled with a sentinel, with a guard gap after the last slot of each plane: hi / lo' are bitwise split_h of
+    the NCHW value the same call wrote, the pad channels +0, every border pixel and the gap untouched; the NCHW result is within TOL of
+    the oracle on all n images.  A plane capacity one slot short is refused before any launch."""
+    import ctypes as C
+    import time
+    from oracle import preprocess as op
+    from stem_plane_checks import sentinel_planes, stem_plane_failures
+    from thinktwice_b200 import lib
+    from thinktwice_b200.preprocess import AgentPreprocessor
+    raw = agent_frames(n, 100 + n)
+    grid = op.undistort_grid((1600, 900))
+    pre = AgentPreprocessor(dict(undistort=True, num_cams=4), CONF, 'cuda:0', map_grid=grid)
+    H0, W0 = CONF['final_dim']
+    pad = (H0 + 6, W0 + 8, 3, 3)                                        # lss.py _single_sweep: 3 px top / bottom / left, 5 right
+    slot = pad[0] * pad[1] * 8
+    split_plane = n * slot + 8 * 4096                                   # guard gap: 4096 pixels after the last slot of each plane
+    planes = sentinel_planes(split_plane, 'cuda')
+    nchw = torch.empty(n, 3, H0, W0, device='cuda')
+    dev = raw.cuda()
+    lib.call('tt_preprocess_u8', C.byref(pre.desc(n, pad)), lib._p(dev), lib._p(pre.grid), lib._p(nchw), lib._p(planes), C.c_longlong(split_plane))
+    torch.cuda.synchronize()
+    bad = stem_plane_failures(planes, split_plane, nchw, pad)
+    assert not bad, bad
+    t0 = time.perf_counter()
+    got, vmax, err = nchw.cpu(), 0.0, 0.0
+    for i in range(0, n, 16):                                           # the oracle in chunks of 16 frames: bounded host memory
+        want = op.image_normalize(op.ida_image_transform(raw[None, i:i + 16], grid, CONF)[0])[0]
+        vmax, err = max(vmax, float(want.abs().max())), max(err, float((got[i:i + 16] - want).abs().max()))
+    print(f'n = {n}: NCHW max error {err:.3g} = {err / vmax:.3g} of max |oracle| (bound {TOL}); oracle on the CPU {time.perf_counter() - t0:.1f} s')
+    assert err <= TOL * vmax
+    # argument checking: planes one slot short of n slots are refused before any launch (and the planes stay as the first call left them)
+    launches = lib.launch_count()
+    rc = lib.load().tt_preprocess_u8(C.byref(pre.desc(n, pad)), lib._p(dev), lib._p(pre.grid), None, lib._p(planes), C.c_longlong(n * slot - slot),
+                                     lib._stream())
+    assert rc == -1 and b'stem-plane capacity' in lib.load().tt_last_error()
+    torch.cuda.synchronize()
+    assert lib.launch_count() == launches
+    assert not stem_plane_failures(planes, split_plane, nchw, pad)
+
+
 def test_lidar_stitch_matches_the_agent_arithmetic():
     from make_preprocess_golden import lidar_case
     from oracle.preprocess import stitch_lidar

@@ -168,6 +168,9 @@ int tt_preprocess_u8(const tt_preproc_desc* d, const uint8_t* raw, const float* 
     TT_REQUIRE(d->pad_top >= 0 && d->pad_left >= 0 && d->pad_top + d->outH <= d->pad_H && d->pad_left + d->outW <= d->pad_W && split_plane % 8 == 0 &&
                    (reinterpret_cast<uintptr_t>(out_split8) & 15) == 0,
                "tt_preprocess_u8", "bad stem-plane geometry");
+  if (out_split8)                                               // n_img padded slots of 8 halves must fit each plane (lo' starts split_plane on)
+    TT_REQUIRE((long long)d->n_img * d->pad_H * d->pad_W * 8 <= split_plane, "tt_preprocess_u8",
+               "n_img stem slots (n_img * pad_H * pad_W * 8 halves) exceed the stem-plane capacity split_plane");
   const long long total = (long long)d->n_img * d->outH * d->outW;
   if (total == 0) return TT_OK;
   const long long want = (total + 255) / 256;

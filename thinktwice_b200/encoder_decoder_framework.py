@@ -228,7 +228,11 @@ class EncoderDecoder(nn.Module):
 
     def attach_preprocessor(self, pre):
         """pre: thinktwice_b200.preprocess.AgentPreprocessor — enables `img_raw` batches (uint8 frames, undistort / resize / crop /
-        normalise fused into the stem's input staging)."""
+        normalise fused into the stem's input staging).  Its final_dim must be the camera encoder's: the f16s engine sizes the stem's
+        slots from the model, so a smaller pre-processed image would fill only a corner of each slot and leave the rest stale."""
+        if pre is not None and (pre.fH, pre.fW) != tuple(self.img_encoder.final_dim):
+            raise lib.TTError(f'the pre-processor produces {pre.fH}x{pre.fW} images, the camera encoder takes '
+                              f'{self.img_encoder.final_dim[0]}x{self.img_encoder.final_dim[1]} (final_dim)')
         self.img_encoder.pre = pre
         return self
 

@@ -147,7 +147,9 @@ class AgentPreprocessor:
         return out
 
     def images_to_stem(self, raw, planes, plane_halves, pad):
-        """raw uint8 device tensor (n, H, W, 3) -> the row-packed stem's operand planes (see tt_image_to_split8); pad = (pad_H, pad_W, top, left)."""
+        """raw uint8 device tensor (n, H, W, 3) -> the row-packed stem's operand planes (see tt_image_to_split8); pad = (pad_H, pad_W, top, left).
+        Frames of another size are refused (TTError), and so are n slots that do not fit a plane of `plane_halves` halves (the C ABI)."""
+        raw = self._raw(raw)
         n = raw.numel() // (self.H * self.W * 3)
         lib.call('tt_preprocess_u8', C.byref(self.desc(n, pad)), _p(raw), _p(self.grid), None, _p(planes), C.c_longlong(plane_halves))
 
