@@ -8,7 +8,8 @@ Per call the harness synchronises, snapshots, runs the entry, synchronises again
   * the elements the contract says are written, against the reference within a per-element bound (or bitwise);
   * every other element of each destination buffer, bitwise unchanged (concat neighbours, pad columns of `ld`, scatter holes, rows of
     a `y_nstride` buffer that belong to other steps);
-  * for the f16s convolutions, that the split planes they write decode to their own fp32 output.
+  * for the f16s convolutions, that the split planes they write decode to their own fp32 output;
+  * for the two loss entries (the open-loop validation forward), that every operand they read is bitwise unchanged.
 Entries that have full-shape checkers of their own are listed in COVERED_ELSEWHERE and only counted; an entry that is in neither map is
 reported, so a new kernel cannot slip in unchecked.
 
@@ -22,11 +23,14 @@ from collections import defaultdict
 
 import torch
 
+import emu_camera_losses
 import emu_frames
 import emu_lib
+import emu_losses
 from emu_lib import IO, NULL, Ptr, _desc, _pix_view, _split_f16, conv_ref, y_region
 
 U = 2.0 ** -24                       # unit roundoff of round-to-nearest fp32
+U64 = 2.0 ** -53                     # ... of fp64 (the loss kernels accumulate in fp64)
 SPLIT = 2.0 ** -22                   # hi + lo'/2048 carries an fp32 value to 2^-22 relative ...
 SPLIT_ABS = 2.0 ** -35               # ... down to the fp16 subnormal step of lo' (2^-24 / 2048)
 MSDA_TOL = 2e-5                      # tests/test_independent_frames_gpu.py: fp32 sample positions, relative to max |ref| of the call
@@ -55,7 +59,7 @@ OUTPUTS = {
     'tt_broadcast_rows': ('y',), 'tt_fill': ('y',), 'tt_maxpool3x3s2': ('y',), 'tt_upsample2x_bilinear_ac': ('y',),
     'tt_global_avgpool': ('y',), 'tt_se_pool': ('s',), 'tt_se_gate': ('y',), 'tt_se_apply': ('y',), 'tt_layernorm': ('y',),
     'tt_eltwise': ('y',), 'tt_msda_forward': ('out',), 'tt_msda_forward_frames': ('out',), 'tt_look_reduce': ('out',),
-    'tt_look_reduce_frames': ('out',),
+    'tt_look_reduce_frames': ('out',), 'tt_loss_reduce': ('out',), 'tt_camera_loss': ('out',),
 }
 IO_FIELDS = ('x_split', 'w_split', 'bias', 'res', 'res_split', 'res2', 'res2_split', 'y', 'y_split')
 CONVS = ('tt_conv2d', 'tt_conv2d_f16s', 'tt_pointwise_f16s')
@@ -128,6 +132,9 @@ class Call:
                         self.p[k] = r
                     else:
                         self.null.add(k)
+        self.decoded = {}                                              # argument name -> fmap -> the argument the reference runs on
+        if name in DECODE:                                             # operands behind pointers inside a table or descriptor
+            DECODE[name](self)
         self.outs = [k for k in OUTPUTS[name] if k in self.p]
         names = [census.namer(self.p[k].t) for k in self.outs]
         self.layer = next((n for n in names if n != 'scratch'), names[0] if names else '?')
@@ -180,6 +187,8 @@ class Call:
         for k, v in self.a.items():
             if k in self.outs:
                 args.append(Ptr(dest[k], self.p[k].off))
+            elif k in self.decoded:
+                args.append(self.decoded[k](fmap))
             elif k in self.p:
                 args.append(self.src_ptr(k, fmap))
             elif k in self.null:
@@ -515,6 +524,195 @@ def bound_eltwise(c, ref, mask):
     return {'y': out}
 
 
+# ---------------------------------------------------------------------------------------------------------- the loss entries
+# tt_loss_reduce and tt_camera_loss read their operands through pointers inside a term table / a descriptor.  DECODE resolves each of
+# those pointers through the census's pointer table (the GPU: an address lib._p handed out since the last checked call; the emulated
+# ABI: the Ptr itself) into an entry of Call.p named after its place ('terms[3].gt', 'd.seg_logits'), so that the operand is
+# snapshotted in fp64 before the call like any other, and rebuilds the table / descriptor over those snapshots for the reference.  A
+# pointer made before an earlier checked call is not in the table any more: the census raises instead of reading a stale buffer.
+LOSS_PTRS = ('pred', 'pred2', 'gt', 'gt2')
+CAM_PTRS = ('seg_logits', 'seg_gt', 'depth_logits', 'depth_gt')
+
+
+def _operand(c, v, what):
+    """a pointer field (an address on the GPU, a Ptr on the emulated ABI) -> its key in c.p, or None for NULL."""
+    r = c.census.resolve(v if isinstance(v, Ptr) else C.c_void_p(v or 0), what)
+    if not r:
+        return None
+    c.p[what] = r
+    return what
+
+
+def decode_loss_terms(c):
+    """tt_loss_reduce: the tt_loss_term array lib.pack_loss_terms built (or, emulated, the term dicts themselves) -> c.terms, term
+    dicts whose pointer fields are keys of c.p; the reference reads them as emu_losses does."""
+    terms = []
+    for i in range(int(emu_lib._v(c.a['n_terms']))):
+        t = c.a['terms'][i]
+        if isinstance(t, dict):
+            d = {k: v for k, v in t.items() if k not in LOSS_PTRS}
+        else:
+            nd = t.ndim
+            d = dict(kind=t.kind, slot=t.slot, aux=t.aux, scale=t.scale, shape=list(t.shape[:nd]), pred_stride=list(t.pred_stride[:nd]),
+                     gt_stride=list(t.gt_stride[:nd]))
+        for f in LOSS_PTRS:
+            d[f] = _operand(c, t[f] if isinstance(t, dict) else getattr(t, f), f'terms[{i}].{f}')
+        terms.append(d)
+    c.terms = terms
+    c.decoded['terms'] = lambda fmap: [dict(t, **{f: c.src_ptr(t[f], fmap) if t[f] else NULL for f in LOSS_PTRS}) for t in terms]
+
+
+def decode_camera_desc(c):
+    """tt_camera_loss: the tt_camera_loss_desc -> a namespace of its fields for emu_camera_losses, pointers over the snapshots.  The
+    ground truth stays fp32 (the kernel bins depths in fp32: an fp64 copy would move values at the bin edges)."""
+    from types import SimpleNamespace
+    from thinktwice_b200 import lib
+    fields = {n: getattr(c.d, n, 0) for n, _ in lib.CameraLossDesc._fields_}
+    keys = {f: _operand(c, fields[f], f'd.{f}') for f in CAM_PTRS}
+    # a logit map is snapshotted as the (pixels, classes) block the kernel reads, not as its whole buffer (a wide map at B = 16 would
+    # pass the working-set cap): the reference reads that block with ld = classes, coff = 0
+    for half, n_cls in (('seg', 'seg_classes'), ('depth', 'depth_bins')):
+        k = keys[f'{half}_logits']
+        if k:
+            rows = fields['BN'] * fields[f'{half}_h'] * fields[f'{half}_w']
+            ld, coff, n = fields[f'{half}_ld'], fields[f'{half}_coff'], fields[n_cls]
+            c.p[k] = Ptr(c.p[k].flat()[:rows * ld].view(rows, ld)[:, coff:coff + n])
+            fields[f'{half}_ld'], fields[f'{half}_coff'] = n, 0
+    fp32 = {k: torch.Tensor.float for f, k in keys.items() if k and f.endswith('_gt')}
+    c.decoded['d'] = lambda fmap: SimpleNamespace(**dict(fields, **{f: c.src_ptr(k, {**fp32, **(fmap or {})}) if k else NULL
+                                                                    for f, k in keys.items()}))
+
+
+DECODE = {'tt_loss_reduce': decode_loss_terms, 'tt_camera_loss': decode_camera_desc}
+
+
+def _digamma_err(x):
+    """|digamma_pos(x) - psi(x)| of csrc/losses.cu, plus the error of the fp64 reference's torch.digamma, for x > 0.
+    digamma_pos takes s = ceil(6 - x) recurrence steps r -= 1 / (x + j) to x' = x + s in [6, 7), then ln x' - 1 / (2x') and the
+    asymptotic series cut after its x'^-10 term.  The series' remainder is smaller than its first dropped term, 691 / (32760 x'^12)
+    (9.7e-12 at x' = 6).  Rounding: the s divisions and subtractions, log, the halving and the 5-term Horner chain in fp64, a few
+    roundings of the magnitude |r| + |ln x'| + 1 each; torch.digamma rounds about as often: 32 u64 of that magnitude."""
+    s = (6.0 - x).ceil().clamp(min=0)
+    xs = x + s
+    mag = xs.log().abs() + 1
+    for j in range(7):
+        mag = mag + torch.where(j < s, 1.0 / (x + j), torch.zeros_like(x))
+    return 691.0 / (32760.0 * xs ** 12) + 32 * U64 * mag
+
+
+def _beta_kl_err(t):
+    """per-element |kernel - reference| bound of a BETA_KL term, both in fp64 (csrc/losses.cu beta_kl; torch's _kl_beta_beta is the same
+    formula): KL = t1 - t2 + (a1 - a2) psi(a1) + (b1 - b2) psi(b1) + (s2 - s1) psi(s1), t1 = lg a2 + lg b2 + lg s1, t2 = lg a1 + lg b1 + lg s2.
+      lgamma: CUDA's is within 4 ulp for x > 0, the reference's about as close; t1 - t2 cancels, so the six lgamma errors and the five
+        sums count as an absolute term in the lgamma magnitudes: 24 u64 (sum |lg| + 6), the + 6 standing for the absolute error an
+        ulp count does not cover near the zeros of lgamma (x = 1, 2);
+      s1 = a1 + b1, s2 = a2 + b2 round once: lgamma moves by |psi(s)| u64 s, psi(s1) by psi'(s1) u64 s1 <= u64 (1 + 1 / s1);
+      each psi: _digamma_err, times the difference it multiplies; the three differences, three products and four sums: 8 u64 of
+      sum |difference psi| and of |KL|."""
+    P, G, P2, G2 = emu_losses.term_operands(t)
+    a1, b1, a2, b2 = G, G2, P, P2
+    s1, s2 = a1 + b1, a2 + b2
+    err = 24 * U64 * (sum(torch.lgamma(x).abs() for x in (a1, b1, s1, a2, b2, s2)) + 6)
+    err = err + U64 * (s1 * torch.digamma(s1).abs() + s2 * torch.digamma(s2).abs()) + (s2 - s1).abs() * U64 * (1 + 1 / s1)
+    for dlt, x in ((a1 - a2, a1), (b1 - b2, b1), (s2 - s1, s1)):
+        err = err + dlt.abs() * (_digamma_err(x) + 8 * U64 * torch.digamma(x).abs())
+    return err
+
+
+def bound_loss_reduce(c, ref, mask):
+    """csrc/losses.cu loss_reduce_kernel, per term of n elements: values v_i in fp64; 16 CTAs of 256 threads each sum ceil(n / 4096)
+    values serially, then an 8-level tree and the 16 range sums serially: a summation depth of ceil(n / 4096) + 24.  The reference's
+    torch sum has depth <= n.  So the two sums differ by at most (ceil(n / 4096) + 24 + n) u64 sum |v_i|, plus sum_i e_i, e_i the
+    two evaluations' error on element i:
+      SMOOTH_L1 (and the clamped form, 1-Lipschitz) / L1: the fp64 |p - g| of two fp32 values (one rounding when their exponents are far
+        apart), 0.5 a a or a - 0.5: 4 u64 |v| each side, 8 u64 |v|;
+      BETA_KL: _beta_kl_err;
+      ACTION_L1: evaluated in fp32 by both as thinktwice_decoder.py:623-636 does (no FMA can change it: x * 2 is exact), and |x1 - x2| in
+        fp64: equal per element, e_i = 0.
+    Then scale * sum and the serial sum over the m terms of the slot: (m + 2) u64 of sum |scale| sum |v|; the slot's fp32 store:
+    U |ref|.  Every slot below n_slots is written (0 when no term names it): the reference's written mask; what is past it must not
+    change."""
+    from thinktwice_b200 import lib
+    n_slots = int(emu_lib._v(c.a['n_slots']))
+    terms = c.decoded['terms'](None)
+    per_slot = defaultdict(int)
+    for t in terms:
+        per_slot[t['slot']] += 1
+    b = torch.zeros(n_slots, dtype=torch.float64, device=ref['out'].device)
+    for t in terms:
+        v = emu_losses.term_values(t)
+        n, A = v.numel(), v.abs().sum()
+        if t['kind'] in (lib.LOSS_SMOOTH_L1, lib.LOSS_SMOOTH_L1_CLAMP, lib.LOSS_L1):
+            e = 8 * U64 * A
+        elif t['kind'] == lib.LOSS_BETA_KL:
+            e = _beta_kl_err(t).sum() + 8 * U64 * A
+        else:
+            e = 0.0
+        b[t['slot']] += abs(t['scale']) * ((math.ceil(n / 4096) + 24 + n + per_slot[t['slot']] + 2) * U64 * A + e)
+    out = torch.zeros_like(ref['out'])
+    o = Ptr(out, c.p['out'].off).flat()
+    o[:n_slots] = b + U * Ptr(ref['out'], c.p['out'].off).flat()[:n_slots].abs()
+    return {'out': out}
+
+
+def bound_camera_loss(c, ref, mask):
+    """csrc/losses.cu camera_loss_kernel against emu_camera_losses, both fp64 up to the final fp32 store.
+    seg_loss: per pixel of C classes, CE = m + log(sum_c exp(q_c - m)) - q_l with the sum in [1, C]: exp and log within 1 ulp, C sums,
+      three more roundings: (C + 8) u64 (2Q + ln C), Q = max_c |q_c|; the N pixels' CEs summed (thread, CTA tree, CTA fold: depth <= N);
+      torch's logsumexp and sum on the reference side the same: |dS| <= 2 (C + N + 8) u64 sum_pixels (2Q + ln C).  ce = S / n rounds
+      once: dce = |dS| / n + u64 ce.  The finish f(ce) = alpha w ce (1 - e^-ce)^gamma (utils.py:43-46) moves by |f'(ce)| dce, doubled
+      for the variation of f' over [ce - dce, ce + dce] (dce / ce is ~1e-12); exp, pow (2 ulp) and four products: 16 u64 |f|.
+    depth_loss: per bin, max(x, 0) - y x + log1p(exp(-|x|)) of magnitude <= 2|x| + 1, within 4 u64 of it; summed over at most
+      BN h w D bins (any order) on either side: |dS| <= 2 (BN h w D + 8) u64 sum_all_bins (2|x| + 1); / max(1, n): + u64 |ref|.
+    Then the fp32 store of each: U |ref|."""
+    d = c.decoded['d'](None)
+    sums = emu_camera_losses.camera_terms(d)
+    r = Ptr(ref['out'], c.p['out'].off).flat()
+    out = torch.zeros_like(ref['out'])
+    o = Ptr(out, c.p['out'].off).flat()
+    if 'seg' in sums:
+        s, n, _, _, _ = sums['seg']
+        BN, h, w, C = d.BN, d.seg_h, d.seg_w, d.seg_classes
+        q = torch.as_strided(d.seg_logits.flat(), (BN, h, w, C), (h * w * d.seg_ld, w * d.seg_ld, d.seg_ld, 1), d.seg_coff)
+        dS = 2 * (C + BN * h * w + 8) * U64 * float((2 * torch.maximum(q.amax(-1), -q.amin(-1)) + math.log(C)).sum())
+        ce = float(s) / max(n, 1)
+        dce = dS / max(n, 1) + U64 * ce
+        g, em = float(d.seg_gamma), math.exp(-ce)
+        fp = float(d.seg_alpha) * float(d.seg_weight) * (1 - em) ** (g - 1) * ((1 - em) + g * ce * em)
+        o[0] = 2 * abs(fp) * dce + (16 * U64 + U) * r[0].abs()
+    if 'depth' in sums:
+        _, n = sums['depth']
+        BN, h, w, D = d.BN, d.depth_h, d.depth_w, d.depth_bins
+        x = torch.as_strided(d.depth_logits.flat(), (BN, h, w, D), (h * w * d.depth_ld, w * d.depth_ld, d.depth_ld, 1), d.depth_coff)
+        dS = 2 * (x.numel() + 8) * U64 * float((2 * x.abs() + 1).sum())
+        o[1] = dS / max(n, 1) + (U64 + U) * r[1].abs()
+    return {'out': out}
+
+
+def check_operands_unchanged(c):
+    """a loss launch may write its destination and its workspace only: every operand it reads is bitwise what it was."""
+    seen = set()
+    for k, p in c.p.items():
+        if k in c.outs or k == 'ws' or id(p.t) in seen:
+            continue
+        seen.add(id(p.t))
+        was = c.src[(id(p.t), None)]
+        now = p.t.to(was.dtype)
+        bad = (now != was) & ~(now.isnan() & was.isnan()) if was.is_floating_point() else now != was
+        if bool(bad.any()):
+            i = int(bad.reshape(-1).nonzero()[0])
+            c.fail(f'{k}: the call changed an operand it only reads: {int(bad.sum())} elements, first {c.where_str(k, i)}')
+
+
+def check_loss(bound_fn):
+    inner = bounded(bound_fn)
+
+    def check(c):
+        inner(c)
+        check_operands_unchanged(c)
+    return check
+
+
 CHECKS = {
     'tt_conv2d': check_conv, 'tt_conv2d_f16s': check_conv, 'tt_pointwise_f16s': check_conv,
     **{k: check_exact for k in ('tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_copy2d', 'tt_anti_transpose', 'tt_nchw_to_nhwc',
@@ -526,6 +724,7 @@ CHECKS = {
     'tt_layernorm': bounded(bound_layernorm), 'tt_eltwise': bounded(bound_eltwise),
     'tt_msda_forward': bounded(bound_msda), 'tt_msda_forward_frames': bounded(bound_msda),
     'tt_look_reduce': bounded(bound_look_reduce), 'tt_look_reduce_frames': bounded(bound_look_reduce),
+    'tt_loss_reduce': check_loss(bound_loss_reduce), 'tt_camera_loss': check_loss(bound_camera_loss),
 }
 assert set(CHECKS) == set(OUTPUTS)
 
@@ -548,12 +747,15 @@ class Census:
     def __init__(self, eng=None, stop=False, outside=True, window=False, cap=None):
         """window: check each convolution on conv_windows (the first and the last images of its N) instead of all of N.  cap: bytes
         of fp64 copies above which a call of another entry is counted as skipped instead of checked."""
-        self.ref = emu_frames.install(emu_lib.Emu())
+        # the loss entries without their lib monkeypatches: the product keeps packing real tt_loss_term arrays / descriptors
+        self.ref = emu_camera_losses.install(emu_losses.install(emu_frames.install(emu_lib.Emu())))
         self.eng, self.stop, self.outside, self.window, self.cap = eng, stop, outside, window, cap
         self.skipped = defaultdict(int)
         self.peak = (0, -1, '')                                        # (bytes, call, entry): the largest working set of one check
+        self.max_allocated = 0                                         # device bytes allocated at most before the latest checked call
         self.calls = 0
         self.stats = {}                                                # entry -> [calls checked, worst ratio, where]
+        self.layers = {}                                               # (entry, layer) -> [calls checked, worst ratio]
         self.failures, self.unchecked, self.covered = [], defaultdict(int), defaultdict(int)
         self.cuda = False
         self._table = None
@@ -633,6 +835,7 @@ class Census:
             self.sync()
             base = 0
             if self.cuda:
+                self.max_allocated = max(self.max_allocated, torch.cuda.max_memory_allocated())
                 base = torch.cuda.memory_allocated()
                 torch.cuda.reset_peak_memory_stats()
             c = Call(self, idx, name, args)
@@ -655,6 +858,9 @@ class Census:
             st[3] = max(st[3], c.planes_ratio)
             if c.ratio >= st[1]:
                 st[1], st[2] = c.ratio, f'call #{idx} [{c.layer}] {c.where}'
+            ls = self.layers.setdefault((name, c.layer), [0, 0.0])
+            ls[0] += 1
+            ls[1] = max(ls[1], c.ratio)
             del c
             if self.cuda:
                 ws = torch.cuda.max_memory_allocated() - base
@@ -681,6 +887,14 @@ class Census:
             lines.append(f'{k:34s} {self.covered[k]:6d} {"elsewhere":>16s}  {COVERED_ELSEWHERE[k]}')
         for k in sorted(self.unchecked):
             lines.append(f'{k:34s} {self.unchecked[k]:6d} {"UNCHECKED":>16s}')
+        return '\n'.join(lines)
+
+    def layer_table(self, prefix):
+        """per (entry, destination buffer) whose buffer name starts with `prefix`: calls checked and the worst err / bound ratio."""
+        lines = [f'{"entry":34s} {"buffer":24s} {"calls":>6s} {"worst err/bound":>16s}']
+        for (k, layer), (n, r) in sorted(self.layers.items()):
+            if layer.startswith(prefix):
+                lines.append(f'{k:34s} {layer:24s} {n:6d} {r:16.3g}')
         return '\n'.join(lines)
 
     def assert_clean(self):
