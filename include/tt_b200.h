@@ -99,7 +99,7 @@ int tt_lift_splat(const tt_lift_splat_desc* d, const float* depth_logits, const 
  * If m_count != NULL only the first *m_count rows (a device int) are computed.
  * `impl`: 0/1 = SIMT fp32 FFMA (exact), 2 = tensor-core single-pass TF32 (operands rounded to nearest TF32),
  *         3 = tensor-core 3xTF32 (hi*hi + hi*lo + lo*hi, fp32-class); 4 = scaled-split fp16 through tt_conv2d_f16s.  impl 2/3 need stride 1 or 2, groups 1, channels,
- *         x_ld, x_coff % 4 == 0 and 16-byte aligned x / w / y (TMA reads the activations in place and splits them in
+ *         x_ld, x_coff, y_ld, y_coff, res_coff, res2_coff and the strides % 4 == 0, 16-byte aligned x / w / y / bias / res / res2 (TMA reads the activations in place and splits them in
  *         shared memory; no workspace); else TT_ERR_UNSUPPORTED.
  *         For impl 0/1 the workspace is optional: when given (size from tt_conv2d_workspace_bytes) small-M / large-K
  *         layers run split-K with a deterministic fixed-order reduction.
@@ -155,7 +155,8 @@ int tt_conv2d_f16s(const tt_conv_desc* d, const tt_f16s_io* io, tt_stream_t stre
  * tt_conv2d impl 0/1 layout) and writes fp32 rows and / or planes.  For maps so large and channels so few that 128 x 64 tensor-core tiles
  * are all overhead (the segmentation head at 224 x 448). */
 int tt_pointwise_f16s(const tt_conv_desc* d, const tt_f16s_io* io, const float* w_kmajor, tt_stream_t stream);
-/* fp32 rows [rows][x_ld] (first `cols` columns) -> split planes [2][rows][y_ld]; only the first *row_count rows when given */
+/* fp32 rows [rows][x_ld] (first `cols` columns) -> split planes [2][rows][y_ld]; only the first *row_count rows when given.  Values are
+ * clamped to +-65504 first (infinities too); a NaN stays NaN in both planes. */
 int tt_split_f16(const float* x, long long x_ld, void* y_split, long long y_plane, long long y_ld, long long rows, int cols,
                  const int* row_count, tt_stream_t stream);
 /* NCHW fp32 images (C <= 8) -> zero-bordered channels-last split planes [2][N][out_H][out_W][8 halves] at pixel offset (top, left): the

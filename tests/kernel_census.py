@@ -88,20 +88,21 @@ def act_bound(act, c, mag, ref):
     return (L * c + a_mag) * U * mag + (1 + a_ref) * U * ref.abs()
 
 
-def conv_c(name, d, K):
+def conv_c(name, d, K, chunk=2):
     """c of the conv bound |y - ref| <= act_bound(c, magnitude), magnitude = conv(|x|, |w|) + |bias| + |res| + |res2|.
 
     tt_conv2d_f16s (csrc/gemm_conv_f16s.cu): the reference reads the decoded split operands, so the only operand error is the
-    dropped lo'·lo' product, |lo'_x lo'_w| / 2048^2 <= 2^-11 |x| 2^-11 |w| = 4 U |x||w|.  Inside the tensor core a K = 128 chunk is
-    8 wgmma k16 steps into a register accumulator that is not rounded to nearest: count 2 ulp (4 U) of the chunk's magnitude per
-    step, doubled for the correction accumulator and its 2^-11 scaling: 64 U per chunk, so 64 U of the whole magnitude.  The fp32
-    register sums add main + 2^-11 corr once per chunk (two roundings) over nc = ceil(K / 128) chunks, and split-K red.add-s at most
-    nc partial sums: 4 nc U.  Bias, two residuals and the fp32 store: 4 U.  So c = 4 + 64 + 4 nc + 4.
+    dropped lo'·lo' product, |lo'_x lo'_w| / 2048^2 <= 2^-11 |x| 2^-11 |w| = 4 U |x||w|.  The register accumulator is folded every
+    `chunk` K stages of 64 (2 by default; 1 / 4 under the debug bits 0x40000 / 0x20000): a fold of 64 chunk K is 4 chunk wgmma
+    k16 steps into an accumulator that is not rounded to nearest: count 2 ulp (4 U) of the fold's magnitude per step, doubled for
+    the correction accumulator and its 2^-11 scaling: 32 chunk U per fold, so 32 chunk U of the whole magnitude.  The fp32 register
+    sums add main + 2^-11 corr once per fold (two roundings) over nc = ceil(K / (64 chunk)) folds, and split-K red.add-s at most
+    nc partial sums: 4 nc U.  Bias, two residuals and the fp32 store: 4 U.  So c = 4 + 32 chunk + 4 nc + 4 (72 + 4 nc at chunk 2).
     tt_pointwise_f16s: the input decoded in fp32 (1 U) and a K-term fp32 FMA chain: c = K + 4.
     tt_conv2d impl 0/1 (SIMT FFMA): K FMA roundings, plus a deterministic split-K reduction of at most K partial sums: c = 2 K + 8;
     impl 2/3 (TF32 pairs) also round the activation operand to 2^-22 (4 U): c = 2 K + 16."""
     if name == 'tt_conv2d_f16s':
-        return 72 + 4 * math.ceil(K / 128)
+        return 8 + 32 * chunk + 4 * math.ceil(K / (64 * chunk))
     if name == 'tt_pointwise_f16s':
         return K + 4
     return 2 * K + (16 if d.impl >= 2 else 8)

@@ -139,10 +139,17 @@ def test_a_count_that_ends_inside_a_tile_ignores_the_stale_rows_past_it(eng, cin
     check(out, out_s, y, bnd, n, cout, f'count mid-tile {cin}->{cout}')
 
 
-@pytest.mark.parametrize('cin,cout', WIDTHS)
-def test_wide_and_narrow_outputs_on_a_random_table_with_more_tiles_than_sms(eng, cin, cout):
+# knobs the output-stationary kernel reads besides 0x200000 / 0x400000: the register fold every 4 / 1 executed stages, and an SM
+# reserve that leaves one CTA to walk every tile ('one-cta': bits 8..15 = SMs - 1, from the device)
+KNOBS = [(0, ''), (0x20000, '-fold4'), (0x40000, '-fold1'), ('one-cta', '-one-cta')]
+
+
+@pytest.mark.parametrize('cin,cout,knobs', [pytest.param(ci, co, k, id=f'{ci}-{co}{tag}') for k, tag in KNOBS for ci, co in WIDTHS])
+def test_wide_and_narrow_outputs_on_a_random_table_with_more_tiles_than_sms(eng, cin, cout, knobs):
     # 20000 rows (157 tiles) of a 27-tap table with mixed occupancy; Cout = 128 runs 128-column tiles, and must agree with the
-    # 64-column tiles debug bit 0x400000 forces; Cout = 32 leaves half of a 64-column tile dead
+    # 64-column tiles debug bit 0x400000 forces; Cout = 32 leaves half of a 64-column tile dead.  The bound does not depend on the fold
+    if knobs == 'one-cta':
+        knobs = (torch.cuda.get_device_properties(0).multi_processor_count - 1) << 8
     g = np.random.default_rng(8)
     n_in, n = 30000, 20000
     dens = np.repeat(g.choice([0.0, 0.05, 0.3, 0.9], n // 128 + 1), 128)[:n, None]
@@ -150,8 +157,8 @@ def test_wide_and_narrow_outputs_on_a_random_table_with_more_tiles_than_sms(eng,
     x_s, x64, w, b = operands(n_in, cin, cout, 27, 9)
     y, bnd = L.expected(ref_nbr(x64, nbr, w), b.numpy(), act=1)
     rb, pw = table_rule(nbr, n, n), L.pack(w.cuda(), b.cuda())
-    out, out_s = L.run_conv(eng, rb, x_s, pw, act=1)
-    a = check(out, out_s, y, bnd, n, cout, f'random {cin}->{cout}')
-    out, out_s = L.run_conv(eng, rb, x_s, pw, act=1, flags=FORCE_BN64)
-    f = check(out, out_s, y, bnd, n, cout, f'random {cin}->{cout} BN 64')
+    out, out_s = L.run_conv(eng, rb, x_s, pw, act=1, flags=knobs)
+    a = check(out, out_s, y, bnd, n, cout, f'random {cin}->{cout} knobs {knobs:#x}')
+    out, out_s = L.run_conv(eng, rb, x_s, pw, act=1, flags=knobs | FORCE_BN64)
+    f = check(out, out_s, y, bnd, n, cout, f'random {cin}->{cout} knobs {knobs:#x} BN 64')
     L.check_conv(a, f.astype(np.float64), 2 * bnd, f'random {cin}->{cout} BN 128 vs 64')

@@ -61,9 +61,13 @@ TT_DEVICE void tma_load_5d(void* dst, const CUtensorMap* map, uint64_t* bar, int
       : "memory");
 }
 
-// x -> (hi, lo') with saturation to the fp16 range; returns true when x had to be clamped
+// x -> (hi, lo') with saturation to the fp16 range; returns true when x had to be clamped (or is NaN).  A NaN stays NaN in both
+// halves, as RN_f16 gives it (fmaxf / fminf would turn it into -65504; the .NaN forms cost the same): tt_split_f16 also sweeps arena
+// rows no kernel has written
 TT_DEVICE bool split_h(float x, __half& hi, __half& lo) {
-  const float c = fminf(fmaxf(x, -H_MAX), H_MAX);
+  float c;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(c) : "f"(x), "f"(-H_MAX));
+  asm("min.NaN.f32 %0, %0, %1;" : "+f"(c) : "f"(H_MAX));
   hi = __float2half_rn(c);
   lo = __float2half_rn((c - __half2float(hi)) * LO_SCALE);
   return c != x;
@@ -656,7 +660,11 @@ __global__ void upsample2x_split_kernel(const float4* __restrict__ x, __half* __
 // 64 x 64 mat-vec at most.  One thread = one pixel: it streams its channel row from the split planes (full 128-byte lines), keeps
 // the COUT accumulators in registers (fp32 FFMA against fp32 weights broadcast from shared memory: exact products, no operand
 // split needed) and stores its output row (fp32 and / or planes).
-template <int COUT>
+// TAIL: Cin % 8 != 0, so the last 8-channel load also reads channels in [Cin, K8), which are not the tensor's (their weights are zero,
+// but the halves there may be NaN: NaN * 0 = NaN) and are zeroed.  YS16: every plane row starts 16-byte aligned (y_ld, y_coff and the
+// plane stride % 8), so a lane stores its 8 halves in one 16-byte store, else in two 8-byte ones.  Both are template parameters: as
+// runtime tests they cost the common case (Cin % 8 == 0, aligned rows) 17-24 % at Cin 64 over 16 x 224 x 448 pixels (H100, 700 W).
+template <int COUT, bool TAIL, bool YS16>
 __global__ void __launch_bounds__(256) pointwise_f16s_kernel(const __half* __restrict__ xs, long long xs_plane, int x_ld, int Cin,
                                                               const float* __restrict__ w, const float* __restrict__ bias, int Cout,
                                                               float* __restrict__ y, __half* __restrict__ ys, long long ys_plane, int y_ld,
@@ -694,6 +702,11 @@ __global__ void __launch_bounds__(256) pointwise_f16s_kernel(const __half* __res
         xv[2 * j] = fmaf(b.x, LO_INV, a.x);
         xv[2 * j + 1] = fmaf(b.y, LO_INV, a.y);
       }
+      if (TAIL && k0 + 8 > Cin) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (k0 + j >= Cin) xv[j] = 0.f;
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float4* wr = reinterpret_cast<const float4*>(&ws[(k0 + j) * COUT]);
@@ -730,9 +743,16 @@ __global__ void __launch_bounds__(256) pointwise_f16s_kernel(const __half* __res
         for (int it = 0; it < 32 / RPI; ++it) {
           const int prow = it * RPI + rsub;
           const long long gp = base + prow;
-          if (gp < npix && co0 + chunk * 8 < Cout)
-            *reinterpret_cast<uint4*>(ys + (pl ? ys_plane : 0) + gp * y_ld + co0 + chunk * 8) =
-                *reinterpret_cast<const uint4*>(&stage[warp][prow * RP + chunk * 16]);
+          if (gp < npix && co0 + chunk * 8 < Cout) {
+            __half* dst = ys + (pl ? ys_plane : 0) + gp * y_ld + co0 + chunk * 8;
+            const uint4 v = *reinterpret_cast<const uint4*>(&stage[warp][prow * RP + chunk * 16]);
+            if (YS16) {
+              *reinterpret_cast<uint4*>(dst) = v;
+            } else {
+              reinterpret_cast<uint2*>(dst)[0] = make_uint2(v.x, v.y);
+              reinterpret_cast<uint2*>(dst)[1] = make_uint2(v.z, v.w);
+            }
+          }
         }
       }
     }
@@ -887,10 +907,20 @@ int tt_pointwise_f16s(const tt_conv_desc* d, const tt_f16s_io* io, const float* 
   float* y = io->y ? io->y + d->y_coff : nullptr;
   if (ys) ys += d->y_coff;
   cudaStream_t st = (cudaStream_t)stream;
+  const bool tail = d->Cin % 8 != 0;
+  const bool ys16 = !ys || (((reinterpret_cast<uintptr_t>(ys) & 15) == 0) && d->y_ld % 8 == 0 && io->y_plane % 8 == 0);
+  auto launch = [&](auto kern, int co0) {
+    kern<<<nb, 256, 0, st>>>(xs, io->x_plane, d->x_ld, d->Cin, w_kmajor, io->bias, d->Cout, y, ys, io->y_plane, d->y_ld, d->act, npix, co0);
+  };
   // 32 output channels per pass (register budget: 2 CTAs per SM); wider layers take two passes over the (small) input rows
   for (int co0 = 0; co0 < d->Cout; co0 += 32) {
-    if (d->Cout <= 16) pointwise_f16s_kernel<16><<<nb, 256, 0, st>>>(xs, io->x_plane, d->x_ld, d->Cin, w_kmajor, io->bias, d->Cout, y, ys, io->y_plane, d->y_ld, d->act, npix, co0);
-    else pointwise_f16s_kernel<32><<<nb, 256, 0, st>>>(xs, io->x_plane, d->x_ld, d->Cin, w_kmajor, io->bias, d->Cout, y, ys, io->y_plane, d->y_ld, d->act, npix, co0);
+    if (d->Cout <= 16) {
+      if (tail) ys16 ? launch(pointwise_f16s_kernel<16, true, true>, co0) : launch(pointwise_f16s_kernel<16, true, false>, co0);
+      else ys16 ? launch(pointwise_f16s_kernel<16, false, true>, co0) : launch(pointwise_f16s_kernel<16, false, false>, co0);
+    } else {
+      if (tail) ys16 ? launch(pointwise_f16s_kernel<32, true, true>, co0) : launch(pointwise_f16s_kernel<32, true, false>, co0);
+      else ys16 ? launch(pointwise_f16s_kernel<32, false, true>, co0) : launch(pointwise_f16s_kernel<32, false, false>, co0);
+    }
     if (co0) ++g_tt_launches;
   }
   ++g_tt_launches;

@@ -448,8 +448,10 @@ bool tt_conv2d_tc_supported(const tt_conv_desc* d, const void* x, const void* w,
   if (d->groups != 1 || (d->stride != 1 && d->stride != 2)) return false;
   if (d->Cin % 4 || d->Cout % 4 || d->x_ld % 4 || d->x_coff % 4 || d->y_ld % 4 || d->x_nstride % 4 || d->y_nstride % 4 || d->x_hstride % 4) return false;
   if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(y)) & 15) return false;
-  if (d->res_mode != TT_RES_NONE && (d->res_ld % 4)) return false;
-  if (d->res2_ld % 4) return false;
+  // the epilogue moves float4 vectors: output and residual channel offsets must keep them 16-byte aligned
+  if (d->y_coff % 4) return false;
+  if (d->res_mode != TT_RES_NONE && (d->res_ld % 4 || d->res_coff % 4)) return false;
+  if (d->res2_ld % 4 || d->res2_coff % 4) return false;
   if (d->OH != (d->H + 2 * d->pad - d->dil * (d->KH - 1) - 1) / d->stride + 1 ||
       d->OW != (d->W + 2 * d->pad - d->dil * (d->KW - 1) - 1) / d->stride + 1) return false;
   return true;
