@@ -468,6 +468,31 @@ typedef struct {
 size_t tt_camera_loss_workspace_bytes(const tt_camera_loss_desc* d);
 int tt_camera_loss(const tt_camera_loss_desc* d, float* out, void* ws, size_t ws_bytes, tt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (12) training-side deformable convolution (SURVEY.md 8f row f4): mmcv's DeformConv2d forward / backward
+ * (mmcv/ops/deform_conv.py, DeformConv2dFunction; the reference builds it at lss.py:189-197) on mmcv's tensors, all contiguous
+ * fp32: input (N, C, H, W), offset (N, 18, H, W) with (dy, dx) interleaved per tap, weight (Cout, C / groups, 3, 3),
+ * output / grad_output (N, Cout, H, W).  Sampling as tt_dcn_im2col: zero unless -1 < h < H and -1 < w < W, out-of-image
+ * corners zero.  Products in 3xTF32 on the tensor cores, fp32 accumulation.
+ * Supported is what the reference builds: 3x3, stride 1, padding 1, dilation 1, deform_groups 1, no bias, C % groups ==
+ * Cout % groups == 0, (C / groups) % 4 == (Cout / groups) % 4 == 0; anything else returns TT_ERR_UNSUPPORTED with the
+ * parameter named in tt_last_error.  Images are processed in chunks of at most im2col_step (the workspace holds one chunk's
+ * columns); output, grad_input and grad_offset do not depend on the chunking.
+ * Backward: grad_input / grad_offset / grad_weight are fully written; any of them may be NULL and is then not computed.
+ * grad_weight and grad_offset are bitwise reproducible (fixed-order reductions); grad_input is accumulated with fp32 atomics.
+ * ws: tt_deform_conv_workspace_bytes(d) bytes of device memory, not shared with a concurrent call.
+ */
+typedef struct {
+  int N, C, H, W, Cout, groups, im2col_step;
+  int kernel_h, kernel_w, stride, padding, dilation, deform_groups;
+} tt_deform_conv_desc;
+size_t tt_deform_conv_workspace_bytes(const tt_deform_conv_desc* d);
+int tt_deform_conv_forward(const tt_deform_conv_desc* d, const float* input, const float* offset, const float* weight, float* output,
+                           void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_deform_conv_backward(const tt_deform_conv_desc* d, const float* input, const float* offset, const float* weight,
+                            const float* grad_output, float* grad_input, float* grad_offset, float* grad_weight, void* ws,
+                            size_t ws_bytes, tt_stream_t stream);
+
 #ifdef __cplusplus
 }
 /* C++ linkage, mangled exactly like the reference's own definition (ops/voxel_pooling/src/voxel_pooling_forward_cuda.cu:38,

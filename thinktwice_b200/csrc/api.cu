@@ -18,7 +18,7 @@ void tt_set_error(const char* fmt, ...) {
 int tt_conv2d_simt(const tt_conv_desc* d, const float* x, const float* w, const float* bias, const float* res,
                    const float* res2, const int* gather, const int* m_count, float* y, void* workspace, cudaStream_t st);
 int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w, const float* bias, const float* res,
-                 const float* res2, float* y, void* workspace, cudaStream_t st);
+                 const float* res2, float* y, void* workspace, cudaStream_t st, bool allow_split_k = true);
 bool tt_conv2d_tc_supported(const tt_conv_desc* d, const void* x, const void* w, const void* y);
 
 extern "C" {

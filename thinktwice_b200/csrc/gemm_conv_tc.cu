@@ -469,8 +469,10 @@ extern "C" size_t tt_conv2d_workspace_bytes(const tt_conv_desc* d) {
 }
 
 // w_tc: [2][Cout][taps][Cin] fp32 = TF32-exact hi plane then lo plane (prepared once per layer by the host).
+// allow_split_k = false keeps every output row's sum in one fixed order (no red.add across K splits): the deformable
+// convolution's outputs must not depend on how many images one call covers.
 int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const float* bias, const float* res,
-                 const float* res2, float* y, void* /*workspace*/, cudaStream_t st) {
+                 const float* res2, float* y, void* /*workspace*/, cudaStream_t st, bool allow_split_k) {
   const int terms = d->impl == 3 ? 3 : 1;
   const int taps = d->KH * d->KW;
   const long long npix_in = (long long)d->N * d->H * d->W;
@@ -532,7 +534,7 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
     const long long tiles = (long long)a.m_tiles * a.n_tiles;
     const bool plain = d->oy_mul == 1 && d->ox_mul == 1 && d->oy_add == 0 && d->ox_add == 0 && d->yH == d->OH && d->yW == d->OW &&
                        d->res_mode != TT_RES_UP2_NEAREST && d->bias_n_mod == 0 && !(g_tt_debug & 128);
-    if (plain && tiles <= num_sms / 2 && k_iters >= 16) {
+    if (allow_split_k && plain && tiles <= num_sms / 2 && k_iters >= 16) {
       int sp = (int)((num_sms + tiles - 1) / tiles);
       if (sp > k_iters / 8) sp = k_iters / 8;
       if (sp > 32) sp = 32;

@@ -98,6 +98,12 @@ class CameraLossDesc(C.Structure):
                [('depth_offset', C.c_float), ('depth_step', C.c_float)]
 
 
+class DeformConvDesc(C.Structure):
+    """tt_deform_conv_desc (include/tt_b200.h section 12): shape and parameters of one deformable convolution."""
+    _fields_ = [(n, C.c_int) for n in ('N', 'C', 'H', 'W', 'Cout', 'groups', 'im2col_step', 'kernel_h', 'kernel_w', 'stride',
+                                        'padding', 'dilation', 'deform_groups')]
+
+
 _lib = None
 
 
@@ -113,7 +119,8 @@ def load():
     lib.tt_last_error.restype = C.c_char_p
     lib.tt_launch_count.restype = C.c_longlong
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
-              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes'):
+              'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
+              'tt_deform_conv_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -130,6 +137,7 @@ EXPORTS = [
     'tt_sparse_conv', 'tt_sparse_to_bev', 'tt_conv2d_f16s', 'tt_split_f16', 'tt_merge_f16', 'tt_image_to_split8', 'tt_pointwise_f16s', 'tt_upsample2x_bilinear_ac_split', 'tt_f16s_saturation_count', 'tt_sparse_conv_f16s', 'tt_sparse_conv_os_f16s', 'tt_look_project', 'tt_look_rebatch', 'tt_msda_forward', 'tt_look_reduce', 'tt_msda_forward_frames', 'tt_look_reduce_frames', 'tt_gru_input',
     'tt_preprocess_u8', 'tt_lidar_stitch', 'tt_points_union', 'tt_voxel_pooling_backward', 'tt_ms_deform_attn_forward', 'tt_ms_deform_attn_backward',
     'tt_loss_workspace_bytes', 'tt_loss_reduce', 'tt_camera_loss_workspace_bytes', 'tt_camera_loss',
+    'tt_deform_conv_workspace_bytes', 'tt_deform_conv_forward', 'tt_deform_conv_backward',
 ]
 
 
