@@ -2,7 +2,8 @@
  * tt_b200.h — C ABI of libtt_b200.so: the H100-native (sm_90a) operator library for the
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
- * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn).
+ * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn), and the training-side
+ * gradients of the native ops on the reference's training step (sections 9, 12 and 13).
  *
  * Conventions (SURVEY.md §8b "External native ABIs"):
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless it says "host";
@@ -492,6 +493,47 @@ int tt_deform_conv_forward(const tt_deform_conv_desc* d, const float* input, con
 int tt_deform_conv_backward(const tt_deform_conv_desc* d, const float* input, const float* offset, const float* weight,
                             const float* grad_output, float* grad_input, float* grad_offset, float* grad_weight, void* ws,
                             size_t ws_bytes, tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (13) training-side sparse convolution (SURVEY.md 8f row f4): spconv 2.x SubMConv3d / SparseConv3d forward and backward, as
+ * mmdet3d's SparseEncoder builds them (lidarnet.py:24-58, cfg thinktwice.py:167-176).  Features are fp32 rows (row pitch in_ld /
+ * out_ld floats), weight (Cout, kvol, Cin) is spconv 2.x's (Cout, kd, kh, kw, Cin) with tap t the row-major flattening of (kd, kh, kw).
+ * For the rulebook's pairs P_t = {(i, o)} of tap t, W_t = weight[:, t, :]:
+ *   y[o] = sum_t sum_{(i,o) in P_t} W_t x[i];  grad_x[i] = sum_t sum_{(i,o) in P_t} W_t^T gy[o];  grad_W_t = sum_{(i,o) in P_t} gy[o] x[i]^T.
+ * Supported is what the reference builds: SubM 3x3x3 (stride 1, padding 1); strided 3x3x3, stride 2, padding 1 or (0, 1, 1);
+ * (3, 1, 1), stride (2, 1, 1), padding 0; dilation 1, groups 1, no bias, not transposed or inverse, kvol <= 32.  Anything else
+ * returns TT_ERR_UNSUPPORTED with the parameter named in tt_last_error.
+ * Forward and grad_input run on the tap-major gather-GEMM of tt_sparse_conv: 3xTF32 tensor cores when Cin, Cout >= 32 (multiples
+ * of 4, pitches multiples of 4, 16-byte aligned rows), fp32 SIMT otherwise; they accumulate over taps with red.add.f32, so they
+ * repeat to fp32 rounding, not bitwise.  grad_weight is a per-tap gathered A-transposed contraction (3xTF32 tensor cores when
+ * Cin, Cout, in_ld, out_ld are multiples of 4, an fp32 SIMT kernel otherwise) folded in a fixed order: bitwise reproducible when
+ * the pair lists are (tt_sparse_pairs_ordered).  The weight is repacked by a kernel in every call (it changes every step).
+ * Row counts stay on the device: rows < *out_count (*in_count) of feats_out (grad_in) are written, the others untouched.
+ */
+typedef struct {
+  int Cin, Cout, kvol;
+  int cap_in, cap_out;           /* row capacities of feats_in / grad_in and feats_out / grad_out */
+  int pair_cap;                  /* pair lists are [kvol][pair_cap]; pair_cap >= the largest tap's pair count */
+  int in_ld, out_ld;             /* row pitches (floats) of the input-side and output-side rows */
+  int k[3], stride[3], padding[3], dilation[3];   /* z, y, x */
+  int subm, groups, bias, transposed, inverse;
+} tt_sparse_conv_train_desc;
+/* 0 when the descriptor is refused (tt_last_error names why); every supported convolution needs a workspace. */
+size_t tt_sparse_conv_train_workspace_bytes(const tt_sparse_conv_train_desc* d);
+int tt_sparse_conv_train_forward(const tt_sparse_conv_train_desc* d, const float* feats_in, const float* weight, const int* pairs_in,
+                                 const int* pairs_out, const int* pair_count, const int* out_count, float* feats_out, void* ws,
+                                 size_t ws_bytes, tt_stream_t stream);
+/* grad_in (rows < *in_count) and grad_weight (Cout, kvol, Cin) are fully written; either may be NULL and is then not computed. */
+int tt_sparse_conv_train_backward(const tt_sparse_conv_train_desc* d, const float* feats_in, const float* weight, const float* grad_out,
+                                  const int* pairs_in, const int* pairs_out, const int* pair_count, const int* in_count,
+                                  const int* out_count, float* grad_in, float* grad_weight, void* ws, size_t ws_bytes,
+                                  tt_stream_t stream);
+/* Pair lists in a fixed order from the neighbour table nbr [cap_out][kvol] of tt_sparse_rulebook (rows >= *out_count are not read):
+ * per tap, the pairs in ascending output row, pairs_in / pairs_out [kvol][pair_cap], pair_count [kvol].  pair_cap must be at least
+ * the largest tap's count (min(input rows, output rows) always is); ws: tt_sparse_pairs_ordered_workspace_bytes(cap_out, kvol). */
+size_t tt_sparse_pairs_ordered_workspace_bytes(int cap_out, int kvol);
+int tt_sparse_pairs_ordered(const int* nbr, const int* out_count, int cap_out, int kvol, int pair_cap, int* pairs_in, int* pairs_out,
+                            int* pair_count, void* ws, size_t ws_bytes, tt_stream_t stream);
 
 #ifdef __cplusplus
 }

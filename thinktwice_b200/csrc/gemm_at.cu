@@ -14,6 +14,10 @@
 //   * split-K: the K range is cut into `splits` contiguous pieces, one CTA per (tile, piece); each writes its partial
 //     tile to the workspace and a fold kernel adds the pieces in piece order.  No floating-point atomics: the result
 //     is bitwise reproducible from run to run on the same GPU.
+// Gather mode (tt_gemm_at_gather, the weight gradient of a sparse convolution): batch b is a kernel tap, row k of A / B is
+// row rows_a[b][k] / rows_b[b][k] of one shared matrix, and K = count[b] is read on the device.  The split count is fixed on
+// the host from the pair capacity; each CTA derives its piece of K from the device count, so no host sync is needed and the
+// fold order stays fixed.  The plain instance the deformable convolution uses is the GATHER = false template.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -32,6 +36,8 @@ struct AtArgs {
   int M, N, K, lda, ldb;
   long long a_batch, b_batch;
   int m_tiles, n_tiles, batch, splits, k_per;   // k_per: K slabs per split
+  const int *rows_a, *rows_b, *count;           // gather mode: [batch][pair_cap] row lists, [batch] K
+  int pair_cap;
 };
 
 TT_DEVICE void split_rn(float x, float& hi, float& lo) {
@@ -41,6 +47,7 @@ TT_DEVICE void split_rn(float x, float& hi, float& lo) {
 TT_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> TT_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
+template <bool GATHER>
 __global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -54,11 +61,15 @@ __global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p) {
   const int mt = t % p.m_tiles;
   const int b = t / p.m_tiles;
   const int i0 = mt * BM, j0 = nt * BN;
-  const int n_slabs_total = (p.K + KS - 1) / KS;
-  const int kb = ks * p.k_per, ke = min(n_slabs_total, kb + p.k_per);
+  const int K = GATHER ? min(__ldg(p.count + b), p.pair_cap) : p.K;
+  const int n_slabs_total = (K + KS - 1) / KS;
+  const int k_per = GATHER ? (n_slabs_total + p.splits - 1) / p.splits : p.k_per;
+  const int kb = ks * k_per, ke = min(n_slabs_total, kb + k_per);
   const int n_it = max(ke - kb, 0);
-  const float* A = p.A + p.a_batch * b;
-  const float* Bm = p.B + p.b_batch * b;
+  const float* A = GATHER ? p.A : p.A + p.a_batch * b;
+  const float* Bm = GATHER ? p.B : p.B + p.b_batch * b;
+  const int* rows_a = GATHER ? p.rows_a + (long long)b * p.pair_cap : nullptr;
+  const int* rows_b = GATHER ? p.rows_b + (long long)b * p.pair_cap : nullptr;
 
   auto load = [&](int it, int s) {                         // slab kb + it -> staging stage s (zero-fill outside K / M / N)
     const int k0 = (kb + it) * KS;
@@ -67,15 +78,17 @@ __global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p) {
     for (int r = 0; r < RAW_A / 16 / NT; ++r) {            // 4 chunks per thread: row k = c / 32, float4 column c % 32
       const int c = tid + r * NT, kk = c >> 5, q = c & 31;
       const int k = k0 + kk, i = i0 + q * 4;
-      const bool ok = k < p.K && i < p.M;
-      cp_async16(ra + c * 16, ok ? A + (long long)k * p.lda + i : p.A, ok ? 16 : 0);
+      const bool ok = k < K && i < p.M;
+      const long long row = GATHER ? (ok ? (long long)__ldg(rows_a + k) : 0) : k;
+      cp_async16(ra + c * 16, ok ? A + row * p.lda + i : p.A, ok ? 16 : 0);
     }
 #pragma unroll
     for (int r = 0; r < RAW_B / 16 / NT; ++r) {            // 2 chunks per thread: row k = c / 16, float4 column c % 16
       const int c = tid + r * NT, kk = c >> 4, q = c & 15;
       const int k = k0 + kk, j = j0 + q * 4;
-      const bool ok = k < p.K && j < p.N;
-      cp_async16(rb + c * 16, ok ? Bm + (long long)k * p.ldb + j : p.B, ok ? 16 : 0);
+      const bool ok = k < K && j < p.N;
+      const long long row = GATHER ? (ok ? (long long)__ldg(rows_b + k) : 0) : k;
+      cp_async16(rb + c * 16, ok ? Bm + row * p.ldb + j : p.B, ok ? 16 : 0);
     }
   };
   // staging stage s -> operand buffer o: transpose to K-major, split into hi / lo, 128-byte swizzle
@@ -217,10 +230,11 @@ int tt_gemm_at(const float* A, int lda, long long a_batch, const float* B, int l
   a.m_tiles = tt_cdiv(M, BM); a.n_tiles = tt_cdiv(N, BN); a.batch = batch;
   a.splits = at_splits(batch, M, N, K);
   a.k_per = tt_cdiv(tt_cdiv(K, KS), a.splits);
+  a.rows_a = a.rows_b = a.count = nullptr; a.pair_cap = 0;
   static bool set = false;
-  if (!set) { cudaFuncSetAttribute(gemm_at_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
   const long long items = (long long)batch * a.m_tiles * a.n_tiles * a.splits;
-  gemm_at_kernel<<<(unsigned)items, NT, SMEM, st>>>(a);
+  gemm_at_kernel<false><<<(unsigned)items, NT, SMEM, st>>>(a);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_gemm_at");
   const long long total = (long long)batch * M * N;
@@ -229,5 +243,38 @@ int tt_gemm_at(const float* A, int lda, long long a_batch, const float* B, int l
                                                                                              c_batch, accumulate);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_gemm_at(fold)");
+  return TT_OK;
+}
+
+// Gather form: C[b][i][j] = sum_{k < count[b]} A[rows_a[b][k]][i] * B[rows_b[b][k]][j] (i < M, j < N), every tap b written (an empty
+// tap gives zeros).  Same tiles, 3xTF32 products and fixed-order fold as tt_gemm_at; ws: tt_gemm_at_workspace_bytes(batch, M, N).
+int tt_gemm_at_gather(const float* A, int lda, const int* rows_a, const float* B, int ldb, const int* rows_b, const int* count, int pair_cap,
+                      float* Cm, int ldc, long long c_batch, int batch, int M, int N, void* ws, size_t ws_bytes, cudaStream_t st) {
+  TT_REQUIRE(A && B && Cm && rows_a && rows_b && count, "tt_gemm_at_gather", "null argument");
+  TT_REQUIRE(M % 4 == 0 && N % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 &&
+                 ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15) == 0,
+             "tt_gemm_at_gather", "M, N, lda and ldb must be multiples of 4 floats, A and B 16-byte aligned");
+  if (batch <= 0 || M <= 0 || N <= 0) return TT_OK;
+  AtArgs a;
+  a.A = A; a.B = B; a.part = static_cast<float*>(ws);
+  a.M = M; a.N = N; a.K = 0; a.lda = lda; a.ldb = ldb; a.a_batch = a.b_batch = 0;
+  a.m_tiles = tt_cdiv(M, BM); a.n_tiles = tt_cdiv(N, BN); a.batch = batch;
+  a.splits = at_splits(batch, M, N, pair_cap > 0 ? pair_cap : 1);   // from the capacity: the counts stay on the device
+  a.k_per = 0;
+  a.rows_a = rows_a; a.rows_b = rows_b; a.count = count; a.pair_cap = pair_cap;
+  TT_REQUIRE(ws && ws_bytes >= (size_t)a.splits * batch * M * N * sizeof(float), "tt_gemm_at_gather",
+             "workspace smaller than tt_gemm_at_workspace_bytes");
+  static bool set = false;
+  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  const long long items = (long long)batch * a.m_tiles * a.n_tiles * a.splits;
+  gemm_at_kernel<true><<<(unsigned)items, NT, SMEM, st>>>(a);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH("tt_gemm_at_gather");
+  const long long total = (long long)batch * M * N;
+  const long long nb = (total + 255) / 256;
+  gemm_at_fold_kernel<<<(int)(nb > tt_num_sms() * 8 ? tt_num_sms() * 8 : nb), 256, 0, st>>>(a.part, a.splits, batch, M, N, Cm, ldc,
+                                                                                             c_batch, 0);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH("tt_gemm_at_gather(fold)");
   return TT_OK;
 }

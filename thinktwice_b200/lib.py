@@ -104,6 +104,13 @@ class DeformConvDesc(C.Structure):
                                         'padding', 'dilation', 'deform_groups')]
 
 
+class SparseConvTrainDesc(C.Structure):
+    """tt_sparse_conv_train_desc (include/tt_b200.h section 13): shape, capacities and parameters of one training-side sparse conv."""
+    _fields_ = [(n, C.c_int) for n in ('Cin', 'Cout', 'kvol', 'cap_in', 'cap_out', 'pair_cap', 'in_ld', 'out_ld')] + \
+               [(n, C.c_int * 3) for n in ('k', 'stride', 'padding', 'dilation')] + \
+               [(n, C.c_int) for n in ('subm', 'groups', 'bias', 'transposed', 'inverse')]
+
+
 _lib = None
 
 
@@ -120,7 +127,7 @@ def load():
     lib.tt_launch_count.restype = C.c_longlong
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
-              'tt_deform_conv_workspace_bytes'):
+              'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -138,6 +145,8 @@ EXPORTS = [
     'tt_preprocess_u8', 'tt_lidar_stitch', 'tt_points_union', 'tt_voxel_pooling_backward', 'tt_ms_deform_attn_forward', 'tt_ms_deform_attn_backward',
     'tt_loss_workspace_bytes', 'tt_loss_reduce', 'tt_camera_loss_workspace_bytes', 'tt_camera_loss',
     'tt_deform_conv_workspace_bytes', 'tt_deform_conv_forward', 'tt_deform_conv_backward',
+    'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_conv_train_forward', 'tt_sparse_conv_train_backward',
+    'tt_sparse_pairs_ordered_workspace_bytes', 'tt_sparse_pairs_ordered',
 ]
 
 
