@@ -3,7 +3,7 @@
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
  * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn), and the training-side
- * gradients of the native ops on the reference's training step (sections 9, 12 and 13).
+ * gradients of the native ops on the reference's training step (sections 9, 12, 13 and 14).
  *
  * Conventions (SURVEY.md §8b "External native ABIs"):
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless it says "host";
@@ -534,6 +534,42 @@ int tt_sparse_conv_train_backward(const tt_sparse_conv_train_desc* d, const floa
 size_t tt_sparse_pairs_ordered_workspace_bytes(int cap_out, int kvol);
 int tt_sparse_pairs_ordered(const int* nbr, const int* out_count, int cap_out, int kvol, int pair_cap, int* pairs_in, int* pairs_out,
                             int* pair_count, void* ws, size_t ws_bytes, tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (14) training-side lift-splat (SURVEY.md 8f row f4): lss.py:583-615 (depth softmax, outer product with the context, frustum
+ * geometry, voxel pooling) with a gradient, on torch's NCHW fp32 tensors and without the (BN, C, D, fH, fW) frustum tensor.
+ * Pixel p of frame b has logits l[p][:], softmax pi[p][:], context f[p][:] and, for bin d, cell(p, d) = y * X + x computed as
+ * tt_lift_splat computes it (bda absent), or -1 outside the grid.  G = dL/dbev.
+ *   forward : bev[b][cell][:] = sum over (p, d) with cell(p, d) = cell of pi[p][d] f[p][:]          (exactly tt_lift_splat)
+ *   backward: g[p][d] = f[p][:] . G[b][:][cell(p, d)] (0 outside the grid);
+ *             grad_logits[p][d] = pi[p][d] (g[p][d] - sum_j pi[p][j] g[p][j]);
+ *             grad_context[p][:] = sum_d pi[p][d] G[b][:][cell(p, d)].
+ *   depth_logits [BN][D][fH][fW] at batch stride depth_bstride floats (so the view depth_feature[:, :D] needs no copy);
+ *   context [BN][C][fH][fW] contiguous; mats / frustum_u / frustum_v / frustum_d as tt_lift_splat.
+ * Forward: bev [B][Y][X][C] is fully overwritten; when bin_cell != NULL it also gets bin_cell [BN*fH*fW][D], the cell the kernel
+ * assigned to every bin or -1: the only state the backward needs besides the inputs.  As tt_lift_splat, the integer-atomic
+ * placement orders each cell's sum differently from run to run (repeatable to fp32 rounding, not bitwise).
+ * Backward: grad_bev (B, C, Y, X) is addressed by ELEMENT strides (any memory order, a channel slice of a concat); the cells are
+ * the recorded bin_cell, never recomputed.  grad_logits [BN][D][fH][fW] and grad_context [BN][C][fH][fW] (contiguous) are fully
+ * written; either may be NULL and is then not computed.  Gathers only, in a fixed order: bitwise reproducible.
+ * Refused with TT_ERR_UNSUPPORTED, the parameter named in tt_last_error, before any pointer or device is touched: D > 128,
+ * C % 4 != 0, C > 512, B*X*Y cells or B*N*fH*fW*D bins past 32-bit indexing, a row tile (C + D) * fW past shared memory, and
+ * ws_bytes < tt_lift_splat_train_workspace_bytes(d).  B = 0 launches nothing.
+ * ws: tt_lift_splat_train_workspace_bytes(d) bytes of device memory (0 when d is refused), not shared with a concurrent call.
+ */
+typedef struct {
+  int B, N, D, fH, fW, C;
+  long long depth_bstride;       /* floats between consecutive images of depth_logits (>= D*fH*fW) */
+  float lower[3], size[3];       /* as tt_lift_splat_desc */
+  int X, Y, Z;
+} tt_lift_splat_train_desc;
+size_t tt_lift_splat_train_workspace_bytes(const tt_lift_splat_train_desc* d);
+int tt_lift_splat_train_forward(const tt_lift_splat_train_desc* d, const float* depth_logits, const float* context, const float* mats,
+                                const float* frustum_u, const float* frustum_v, const float* frustum_d, float* bev, int* bin_cell,
+                                void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_lift_splat_train_backward(const tt_lift_splat_train_desc* d, const float* depth_logits, const float* context, const int* bin_cell,
+                                 const float* grad_bev, long long stride_b, long long stride_c, long long stride_y, long long stride_x,
+                                 float* grad_logits, float* grad_context, void* ws, size_t ws_bytes, tt_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -111,6 +111,12 @@ class SparseConvTrainDesc(C.Structure):
                [(n, C.c_int) for n in ('subm', 'groups', 'bias', 'transposed', 'inverse')]
 
 
+class LiftSplatTrainDesc(C.Structure):
+    """tt_lift_splat_train_desc (include/tt_b200.h section 14): shapes, logits batch stride and voxel grid of the training lift-splat."""
+    _fields_ = [(n, C.c_int) for n in ('B', 'N', 'D', 'fH', 'fW', 'C')] + [('depth_bstride', C.c_longlong)] + \
+               [('lower', C.c_float * 3), ('size', C.c_float * 3)] + [(n, C.c_int) for n in ('X', 'Y', 'Z')]
+
+
 _lib = None
 
 
@@ -127,7 +133,8 @@ def load():
     lib.tt_launch_count.restype = C.c_longlong
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
-              'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes'):
+              'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes',
+              'tt_lift_splat_train_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -147,6 +154,7 @@ EXPORTS = [
     'tt_deform_conv_workspace_bytes', 'tt_deform_conv_forward', 'tt_deform_conv_backward',
     'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_conv_train_forward', 'tt_sparse_conv_train_backward',
     'tt_sparse_pairs_ordered_workspace_bytes', 'tt_sparse_pairs_ordered',
+    'tt_lift_splat_train_workspace_bytes', 'tt_lift_splat_train_forward', 'tt_lift_splat_train_backward',
 ]
 
 
