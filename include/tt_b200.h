@@ -3,7 +3,7 @@
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
  * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn), and the training-side
- * gradients of the native ops on the reference's training step (sections 9, 12, 13 and 14).
+ * gradients of the native ops and losses on the reference's training step (sections 9, 10b, 12, 13, 14 and 15).
  *
  * Conventions (SURVEY.md §8b "External native ABIs"):
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless it says "host";
@@ -440,6 +440,29 @@ typedef struct {
  * on `stream`); ws: tt_loss_workspace_bytes(n_terms) bytes of device memory, not shared with a concurrent call. */
 size_t tt_loss_workspace_bytes(int n_terms);
 int tt_loss_reduce(const tt_loss_term* terms, int n_terms, float* out, int n_slots, void* ws, size_t ws_bytes, tt_stream_t stream);
+/* (10b) the decoder terms' gradient (training side, SURVEY.md 8f row f4).  grads[k] goes with terms[k] (the same table tt_loss_reduce
+ * reads).  Term k's upstream gradient is u_k = sum of grad_out[up_slot .. up_slot + up_count) in slot order (fp64), so a (B, 1) loss
+ * whose slots all feed one term (value_loss's pred_value_traj mean) needs one term, and a term fed by one frame's slot needs count 1.
+ * With d = pred - gt and s(d) = clamp(d, -1, 1) (torch's smooth_l1 backward, beta 1; NaN stays NaN), every element of the term gets
+ *   SMOOTH_L1       : grad_pred = u * scale * s(d)
+ *   SMOOTH_L1_CLAMP : grad_pred = (-5 <= smooth_l1(d) <= 5 ? u : 0) * scale * s(d)   (torch.clamp's backward passes the bounds)
+ *   BETA_KL         : grad_pred  = u * scale * (psi(a2) - psi(a2 + b2) - psi(a1) + psi(a1 + b1)),
+ *                     grad_pred2 = u * scale * (psi(b2) - psi(a2 + b2) - psi(b1) + psi(a1 + b1)),  a1, b1 = gt, gt2; a2, b2 = pred, pred2
+ * in fp64, rounded once.  A term with grad_pred NULL is skipped; L1 and ACTION_L1 terms (computed under no_grad by the reference) with
+ * a gradient pointer are refused.  Refused with TT_ERR_UNSUPPORTED (the reason in tt_last_error) before anything is staged: a gradient
+ * view that maps two elements to one address, and two terms (or grad_pred / grad_pred2 of one term) whose gradient address ranges
+ * [lowest, highest element] intersect.  So every gradient element is written by exactly one thread, once, without atomics: bitwise
+ * reproducible.  Elements no term covers are not written.  `terms` / `grads` are HOST memory (copied into ws on `stream`); grad_out
+ * [n_slots] is device memory; ws: tt_loss_backward_workspace_bytes(n_terms) bytes, not shared with a concurrent call. */
+typedef struct {
+  float* grad_pred;             /* dL/dpred over the term's shape at grad_stride; NULL: no gradient for this term */
+  float* grad_pred2;            /* BETA_KL: dL/dpred2 at the same strides (may be NULL); otherwise unused */
+  long long grad_stride[TT_LOSS_MAX_DIM];
+  int up_slot, up_count;        /* upstream gradient = sum of grad_out[up_slot .. up_slot + up_count) */
+} tt_loss_grad;
+size_t tt_loss_backward_workspace_bytes(int n_terms);
+int tt_loss_backward(const tt_loss_term* terms, int n_terms, const tt_loss_grad* grads, const float* grad_out, int n_slots, void* ws,
+                     size_t ws_bytes, tt_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * (11) the camera branch's supervision of the key frame (encoder_decoder_framework.py:171-190, 442-491; utils.py:31-47):
@@ -570,6 +593,51 @@ int tt_lift_splat_train_forward(const tt_lift_splat_train_desc* d, const float* 
 int tt_lift_splat_train_backward(const tt_lift_splat_train_desc* d, const float* depth_logits, const float* context, const int* bin_cell,
                                  const float* grad_bev, long long stride_b, long long stride_c, long long stride_y, long long stride_x,
                                  float* grad_logits, float* grad_context, void* ws, size_t ws_bytes, tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (15) training-side camera supervision (SURVEY.md 8f row f4): section 11's seg_loss / depth_loss with a gradient, on torch's NCHW fp32
+ * logits (encoder_decoder_framework.py:171-190).  Ground truth, quirks and sums are tt_camera_loss's: labels read at ATen's nearest
+ * index and truncated by .long(); depth 0 -> 1e5 before the min-pool; a NaN pixel makes its block background; the focal transform of
+ * the batch-MEAN cross entropy; fixed-order fp64 sums folded by the last CTA, bitwise reproducible.
+ * Logits: class / bin c of pixel (n, y, x) at logits[n * stride[0] + c * stride[1] + y * stride[2] + x * stride[3]]; the h x w plane
+ * must be dense (stride[3] = 1, stride[2] = w), so the seg head's output and the view depth_feature[:, :D] pass without a copy.
+ * Forward: out[0] = seg_loss, out[1] = depth_loss (a half that is off leaves its slot untouched), and *stats (device memory).  When
+ * seg_target / depth_target are non-NULL it also records the target of every logit pixel: seg_target [BN][seg_h][seg_w] = the class,
+ * or 255 for an ignored pixel (or a label torch rejects); depth_target [BN][depth_h][depth_w] = the bin 1..depth_bins, or 0 for a
+ * background cell.  The backward reads these records and *stats, never the ground truth.
+ * Backward: grad_loss = (dL/dseg_loss, dL/ddepth_loss), 2 device floats.  With k0 = grad_loss[0] * stats->seg_factor and
+ * k1 = grad_loss[1] / max(1, nfg):
+ *   grad_seg  [BN][C][seg_h][seg_w]   = k0 * (softmax_c(p) - [c = label(p)]) on counted pixels, 0 on ignored pixels;
+ *   grad_depth[BN][D][depth_h][depth_w] = k1 * (sigmoid(x_pd) - [d = bin(p) - 1]) on foreground cells, 0 on background cells;
+ * both contiguous NCHW and fully written; either may be NULL and is then skipped.  Element-wise, no atomics: bitwise reproducible.
+ * Refused with TT_ERR_UNSUPPORTED, the parameter named in tt_last_error, before any pointer is touched: seg_classes > 32 (the
+ * backward's register tile), depth_bins > 255 (a byte target), a plane that is not dense, pixel / cell / ground-truth counts past
+ * 32-bit indexing, and (forward) ws_bytes < tt_camera_loss_train_workspace_bytes(d).  BN = 0 launches nothing and writes nothing.
+ */
+typedef struct {
+  const float* seg_logits;      /* (BN, seg_classes, seg_h, seg_w) at seg_stride; NULL: no seg_loss */
+  const float* seg_gt;          /* (BN, seg_H, seg_W) labels as floats, as tt_camera_loss_desc */
+  const float* depth_logits;    /* (BN, depth_bins, depth_h, depth_w) at depth_stride; NULL: no depth_loss */
+  const float* depth_gt;        /* (BN, depth_h * depth_factor, depth_w * depth_factor) depths */
+  long long seg_stride[4];      /* element strides of (n, c, y, x) */
+  long long depth_stride[4];
+  int BN;
+  int seg_h, seg_w, seg_H, seg_W, seg_classes, seg_ignore;
+  float seg_alpha, seg_gamma, seg_weight;
+  int depth_h, depth_w, depth_factor, depth_bins;
+  float depth_offset, depth_step;  /* as tt_camera_loss_desc */
+} tt_camera_loss_train_desc;
+typedef struct {
+  double ce;                    /* mean cross entropy over the counted pixels (NaN: none counted, or a rejected label) */
+  double seg_factor;            /* seg_weight * f'(ce) / nseg, f(ce) = alpha * ce * (1 - e^-ce)^gamma: d seg_loss / d CE sum */
+  long long nseg, nfg, bad;     /* counted pixels / foreground cells / labels torch rejects */
+} tt_camera_loss_stats;
+size_t tt_camera_loss_train_workspace_bytes(const tt_camera_loss_train_desc* d);
+int tt_camera_loss_train_forward(const tt_camera_loss_train_desc* d, float* out, tt_camera_loss_stats* stats, uint8_t* seg_target,
+                                 uint8_t* depth_target, void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_camera_loss_train_backward(const tt_camera_loss_train_desc* d, const tt_camera_loss_stats* stats, const uint8_t* seg_target,
+                                  const uint8_t* depth_target, const float* grad_loss, float* grad_seg, float* grad_depth,
+                                  tt_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -89,6 +89,12 @@ class LossTerm(C.Structure):
                 ('ndim', C.c_int), ('kind', C.c_int), ('slot', C.c_int), ('aux', C.c_int), ('scale', C.c_double)]
 
 
+class LossGrad(C.Structure):
+    """tt_loss_grad (include/tt_b200.h section 10b): the gradient outputs and upstream slots of one term of tt_loss_backward."""
+    _fields_ = [('grad_pred', C.c_void_p), ('grad_pred2', C.c_void_p), ('grad_stride', C.c_longlong * LOSS_MAX_DIM),
+                ('up_slot', C.c_int), ('up_count', C.c_int)]
+
+
 class CameraLossDesc(C.Structure):
     """tt_camera_loss_desc (include/tt_b200.h section 11): the segmentation and depth halves of tt_camera_loss."""
     _fields_ = [('seg_logits', C.c_void_p), ('seg_gt', C.c_void_p), ('depth_logits', C.c_void_p), ('depth_gt', C.c_void_p), ('BN', C.c_int)] + \
@@ -117,6 +123,21 @@ class LiftSplatTrainDesc(C.Structure):
                [('lower', C.c_float * 3), ('size', C.c_float * 3)] + [(n, C.c_int) for n in ('X', 'Y', 'Z')]
 
 
+class CameraLossTrainDesc(C.Structure):
+    """tt_camera_loss_train_desc (include/tt_b200.h section 15): the two halves of the training camera supervision on NCHW logits."""
+    _fields_ = [('seg_logits', C.c_void_p), ('seg_gt', C.c_void_p), ('depth_logits', C.c_void_p), ('depth_gt', C.c_void_p),
+                ('seg_stride', C.c_longlong * 4), ('depth_stride', C.c_longlong * 4), ('BN', C.c_int)] + \
+               [(n, C.c_int) for n in ('seg_h', 'seg_w', 'seg_H', 'seg_W', 'seg_classes', 'seg_ignore')] + \
+               [(n, C.c_float) for n in ('seg_alpha', 'seg_gamma', 'seg_weight')] + \
+               [(n, C.c_int) for n in ('depth_h', 'depth_w', 'depth_factor', 'depth_bins')] + \
+               [('depth_offset', C.c_float), ('depth_step', C.c_float)]
+
+
+class CameraLossStats(C.Structure):
+    """tt_camera_loss_stats (include/tt_b200.h section 15): what the training camera forward leaves on the device for its backward."""
+    _fields_ = [('ce', C.c_double), ('seg_factor', C.c_double), ('nseg', C.c_longlong), ('nfg', C.c_longlong), ('bad', C.c_longlong)]
+
+
 _lib = None
 
 
@@ -134,7 +155,7 @@ def load():
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
               'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes',
-              'tt_lift_splat_train_workspace_bytes'):
+              'tt_lift_splat_train_workspace_bytes', 'tt_loss_backward_workspace_bytes', 'tt_camera_loss_train_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -155,6 +176,8 @@ EXPORTS = [
     'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_conv_train_forward', 'tt_sparse_conv_train_backward',
     'tt_sparse_pairs_ordered_workspace_bytes', 'tt_sparse_pairs_ordered',
     'tt_lift_splat_train_workspace_bytes', 'tt_lift_splat_train_forward', 'tt_lift_splat_train_backward',
+    'tt_loss_backward_workspace_bytes', 'tt_loss_backward',
+    'tt_camera_loss_train_workspace_bytes', 'tt_camera_loss_train_forward', 'tt_camera_loss_train_backward',
 ]
 
 
@@ -168,6 +191,16 @@ def pack_loss_terms(terms):
         a.ndim, a.kind, a.slot, a.aux, a.scale = len(t['shape']), t['kind'], t['slot'], t['aux'], t['scale']
         for d, (n, ps, gs) in enumerate(zip(t['shape'], t['pred_stride'], t['gt_stride'])):
             a.shape[d], a.pred_stride[d], a.gt_stride[d] = n, ps, gs
+    return arr
+
+
+def pack_loss_grads(grads):
+    """list of gradient dicts (LossGrad's field names; pointers from `_p`) -> the tt_loss_grad array tt_loss_backward reads."""
+    arr = (LossGrad * len(grads))()
+    for a, g in zip(arr, grads):
+        a.grad_pred, a.grad_pred2, a.up_slot, a.up_count = g['grad_pred'], g['grad_pred2'], g['up_slot'], g['up_count']
+        for d, s in enumerate(g['grad_stride']):
+            a.grad_stride[d] = s
     return arr
 
 
