@@ -84,13 +84,23 @@ TT_DEVICE void split4(const float4& o, uint2& hi, uint2& lo, bool& sat) {
   lo.y = (uint32_t)__half_as_ushort(l[2]) | ((uint32_t)__half_as_ushort(l[3]) << 16);
 }
 
-TT_DEVICE float4 load_split4(const __half* hi_ptr, long long plane) {
-  const uint2 h = *reinterpret_cast<const uint2*>(hi_ptr);
-  const uint2 l = *reinterpret_cast<const uint2*>(hi_ptr + plane);
+// four hi / lo' pairs -> fp32 (hi + lo' 2^-11)
+TT_DEVICE float4 merge_split4(const uint2& h, const uint2& l) {
   const __half2 h0 = *reinterpret_cast<const __half2*>(&h.x), h1 = *reinterpret_cast<const __half2*>(&h.y);
   const __half2 l0 = *reinterpret_cast<const __half2*>(&l.x), l1 = *reinterpret_cast<const __half2*>(&l.y);
   const float2 a = __half22float2(h0), b = __half22float2(h1), c = __half22float2(l0), e = __half22float2(l1);
   return make_float4(fmaf(c.x, LO_INV, a.x), fmaf(c.y, LO_INV, a.y), fmaf(e.x, LO_INV, b.x), fmaf(e.y, LO_INV, b.y));
+}
+TT_DEVICE float4 load_split4(const __half* hi_ptr, long long plane) {
+  return merge_split4(*reinterpret_cast<const uint2*>(hi_ptr), *reinterpret_cast<const uint2*>(hi_ptr + plane));
+}
+
+// tt_act over four values with one test of the (kernel-uniform) activation for the inline cases: tested per element, the out-of-line
+// call of the rare activations put two compares and three branches around every value of the epilogue
+TT_DEVICE float4 act4(const float4& o, int act) {
+  if (act == TT_ACT_NONE) return o;
+  if (act == TT_ACT_RELU) return make_float4(fmaxf(o.x, 0.f), fmaxf(o.y, 0.f), fmaxf(o.z, 0.f), fmaxf(o.w, 0.f));
+  return make_float4(tt_act(o.x, act), tt_act(o.y, act), tt_act(o.z, act), tt_act(o.w, act));
 }
 
 struct HArgs {
@@ -138,7 +148,9 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
   constexpr int SLAB = 16;                                // epilogue column slab
   constexpr int PITCH = SLAB + 4;                         // +4 floats: conflict-free transposition
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // rounded up to 1 KB as an offset from smem_raw, not through an integer: the compiler then keeps the shared address space, and the
+  // epilogue's transposition compiles to shared-memory loads and stores instead of generic ones
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   float* tile_all = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);              // [8 MMA warps][16 rows][PITCH]
   uint64_t* bars = reinterpret_cast<uint64_t*>(tile_all + 8 * 16 * PITCH);
   uint64_t* full = bars;                                  // [STAGES]  producer -> MMA (operands landed)
@@ -469,26 +481,48 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           fl[i] = (valid ? 1 : 0) | (nimg << 1);
         }
       }
-      // ---- coalesced store in 16-column slabs: registers -> warp-private smem (transpose) -> 64-byte row segments
+      // ---- residual and bias strip: the loads for all BN / 16 slabs are issued before the first slab is stored, so that a thread
+      // has its whole strip in flight at once instead of paying one memory round trip per 16 columns (acc[] / cor[] are dead here,
+      // which leaves the registers).  A split residual stays as its raw hi / lo' halves until it is used.
+      constexpr int NSL = BN / SLAB;
+      const bool res_split = !p.res && p.res_s;
+      uint4 rv[NSL][2];                                       // fp32 residual bits, or split (hi.x, hi.y, lo.x, lo.y); 0 = none
+      float4 bv[NSL];                                         // bias vector; per-image rows (bias_n_mod) are loaded per slab below
 #pragma unroll
-      for (int sl = 0; sl < BN / SLAB; ++sl) {
+      for (int sl = 0; sl < NSL; ++sl) {
         const int col = n0 + sl * SLAB + cl;
         const bool live = col < d.Cout;
-        // residual / bias loads of this slab are issued BEFORE the shared-memory transposition so that the two latencies overlap
-        float4 ra[2], rb[2];
-        float4 bv0 = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-          ra[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          rb[i] = ra[i];
+          rv[sl][i] = make_uint4(0u, 0u, 0u, 0u);
           if (live && (fl[i] & 1)) {
-            if (p.res) ra[i] = *reinterpret_cast<const float4*>(p.res + o1[i] + col);
-            else if (p.res_s) ra[i] = load_split4(p.res_s + o1[i] + col, p.res_plane);
+            if (p.res) {
+              rv[sl][i] = *reinterpret_cast<const uint4*>(p.res + o1[i] + col);
+            } else if (p.res_s) {
+              const uint2 h = *reinterpret_cast<const uint2*>(p.res_s + o1[i] + col);
+              const uint2 l = *reinterpret_cast<const uint2*>(p.res_s + p.res_plane + o1[i] + col);
+              rv[sl][i] = make_uint4(h.x, h.y, l.x, l.y);
+            }
+          }
+        }
+        bv[sl] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (live && p.bias && !d.bias_n_mod) bv[sl] = __ldg(reinterpret_cast<const float4*>(p.bias + col));
+      }
+      // ---- coalesced store in 16-column slabs: registers -> warp-private smem (transpose) -> 64-byte row segments
+#pragma unroll
+      for (int sl = 0; sl < NSL; ++sl) {
+        const int col = n0 + sl * SLAB + cl;
+        const bool live = col < d.Cout;
+        // second residual and bias_n_mod rows: per slab (a second strip spills at BN = 128); issued before the transposition to overlap it
+        float4 rb[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (live && (fl[i] & 1)) {
             if (p.res2) rb[i] = *reinterpret_cast<const float4*>(p.res2 + o2[i] + col);
             else if (p.res2_s) rb[i] = load_split4(p.res2_s + o2[i] + col, p.res2_plane);
           }
         }
-        if (live && p.bias && !d.bias_n_mod) bv0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));   // one bias vector: once per slab
         __syncwarp();
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj) {                     // fragment column group j = 2 sl + jj: columns 8 jj + 2 (lane % 4) + {0, 1}
@@ -502,15 +536,18 @@ conv_f16s_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           for (int i = 0; i < 2; ++i) {
             if (!(fl[i] & 1)) continue;
             const float4 acc4 = *reinterpret_cast<const float4*>(&tile[(i * 8 + sub) * PITCH + cl]);
-            float4 bv = bv0;
-            if (p.bias && d.bias_n_mod) bv = __ldg(reinterpret_cast<const float4*>(p.bias + (long long)((fl[i] >> 1) % d.bias_n_mod) * d.Cout + col));
-            float4 o = make_float4(acc4.x + bv.x + ra[i].x + rb[i].x, acc4.y + bv.y + ra[i].y + rb[i].y,
-                                   acc4.z + bv.z + ra[i].z + rb[i].z, acc4.w + bv.w + ra[i].w + rb[i].w);
+            float4 b = bv[sl];
+            if (p.bias && d.bias_n_mod) b = __ldg(reinterpret_cast<const float4*>(p.bias + (long long)((fl[i] >> 1) % d.bias_n_mod) * d.Cout + col));
+            const uint4 r = rv[sl][i];
+            const float4 ra = res_split ? merge_split4(make_uint2(r.x, r.y), make_uint2(r.z, r.w))
+                                        : make_float4(__uint_as_float(r.x), __uint_as_float(r.y), __uint_as_float(r.z), __uint_as_float(r.w));
+            float4 o = make_float4(acc4.x + b.x + ra.x + rb[i].x, acc4.y + b.y + ra.y + rb[i].y,
+                                   acc4.z + b.z + ra.z + rb[i].z, acc4.w + b.w + ra.w + rb[i].w);
             const long long eo = yo[i] + col;
             if (GM == 1 || p.splits > 1) {                     // taps / K splits race on an output row: red.add (fp32 only)
               tt_red_add_v4(p.y + eo, o.x, o.y, o.z, o.w);
             } else {
-              o = make_float4(tt_act(o.x, d.act), tt_act(o.y, d.act), tt_act(o.z, d.act), tt_act(o.w, d.act));
+              o = act4(o, d.act);
               if (p.y) *reinterpret_cast<float4*>(p.y + eo) = o;
               if (p.ys) {
                 uint2 hi, lo;
