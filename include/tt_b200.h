@@ -3,7 +3,7 @@
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
  * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn), and the training-side
- * gradients of the native ops and losses on the reference's training step (sections 9, 10b, 12, 13, 14 and 15).
+ * gradients of the native ops, losses and dense convolutions on the reference's training step (sections 9, 10b and 12 to 16).
  *
  * Conventions (SURVEY.md §8b "External native ABIs"):
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless it says "host";
@@ -638,6 +638,41 @@ int tt_camera_loss_train_forward(const tt_camera_loss_train_desc* d, float* out,
 int tt_camera_loss_train_backward(const tt_camera_loss_train_desc* d, const tt_camera_loss_stats* stats, const uint8_t* seg_target,
                                   const uint8_t* depth_target, const float* grad_loss, float* grad_seg, float* grad_depth,
                                   tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (16) training-side dense convolution (SURVEY.md 2.2 N6): torch.nn.Conv2d forward and backward, for the layers a training step
+ * puts through forward and backward (the camera trunk with frozen_stages=-1, the DepthNet, the seg head, the BEV fusion, SECOND).
+ *   y[n][oh][ow][o] = bias[o] + sum_{i, kh, kw} weight[o][i][kh][kw] x[n][oh * stride - pad + kh * dil][ow * stride - pad + kw * dil][i]
+ * with out-of-image input pixels zero.  Activations and their gradients in torch's channels_last storage: x, grad_x [N][H][W][Cin],
+ * y, grad_y [N][OH][OW][Cout]; weight, grad_weight torch's contiguous (Cout, Cin, KH, KW); bias, grad_bias [Cout].  Products in
+ * 3xTF32 on the tensor cores (fp32-class over fp32's whole exponent range), fp32 accumulation.  The weight is repacked by a kernel
+ * in every call (it changes every optimiser step).
+ *   forward : the implicit-GEMM tensor-core convolution, bias in its epilogue;
+ *   grad_x  : stride 1, one convolution of grad_y with the flipped, transposed kernel; stride 2, one stride-1 convolution per output
+ *             phase (y mod 2, x mod 2) with the sub-kernel of the taps that reach it, stored through a pixel scatter; pixels no tap
+ *             reaches are written as zeros.  No im2col, no zero-inserted copy of grad_y;
+ *   grad_weight: per tap, grad_y^T x(shifted) as a contraction over the output pixels (A-transposed tensor-core GEMM), split over
+ *             pixels and folded in a fixed order;
+ *   grad_bias: per-channel sum of grad_y over the pixels in fixed chunks, folded in a fixed order.
+ * Determinism: y, grad_x, grad_weight and grad_bias are each bitwise reproducible from run to run on the same GPU (no split-K with
+ * red.add, no floating-point atomics).
+ * Supported: groups 1, stride 1 or 2, Cin and Cout multiples of 4, any kernel size, padding >= 0 and dilation >= 1, OH / OW equal
+ * to (H + 2 pad - dil (KH - 1) - 1) / stride + 1 (resp. W, KW) and at least 1, pixel and element counts within 32-bit indexing.
+ * Anything else, and ws_bytes < tt_conv2d_train_workspace_bytes(d), returns TT_ERR_UNSUPPORTED with the parameter named in
+ * tt_last_error, before any pointer or device is touched.  N = 0 launches no kernel (grad_weight / grad_bias are zeroed by memset).
+ * Forward: y is fully written; bias is read when d->bias (NULL otherwise).  Backward: grad_x, grad_weight and grad_bias (when
+ * d->bias) are fully written; any of them may be NULL and is then not computed.
+ * ws: tt_conv2d_train_workspace_bytes(d) bytes of device memory, not shared with a concurrent call.
+ */
+typedef struct {
+  int N, H, W, Cin, Cout, KH, KW, stride, pad, dil, groups, bias;
+  int OH, OW;
+} tt_conv2d_train_desc;
+size_t tt_conv2d_train_workspace_bytes(const tt_conv2d_train_desc* d);   /* 0 when refused */
+int tt_conv2d_train_forward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* bias, float* y,
+                            void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_conv2d_train_backward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* grad_y,
+                             float* grad_x, float* grad_weight, float* grad_bias, void* ws, size_t ws_bytes, tt_stream_t stream);
 
 #ifdef __cplusplus
 }

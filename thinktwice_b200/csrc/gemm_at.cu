@@ -17,7 +17,11 @@
 // Gather mode (tt_gemm_at_gather, the weight gradient of a sparse convolution): batch b is a kernel tap, row k of A / B is
 // row rows_a[b][k] / rows_b[b][k] of one shared matrix, and K = count[b] is read on the device.  The split count is fixed on
 // the host from the pair capacity; each CTA derives its piece of K from the device count, so no host sync is needed and the
-// fold order stays fixed.  The plain instance the deformable convolution uses is the GATHER = false template.
+// fold order stays fixed.  The plain instance the deformable convolution uses is the MODE = AT_PLAIN template.
+// Conv mode (tt_gemm_at_conv, the weight gradient of a dense convolution): batch b is tap (kh, kw), row k of A is pixel k of the
+// output gradient [P][M] and row k of B is the input pixel (n, oh * stride - pad + kh * dil, ow * stride - pad + kw * dil) of the
+// channels-last input [N][H][W][N cols], zero-filled (cp.async src-size 0) when it falls outside the image.  Its fold writes the
+// torch weight layout (M, N, KH, KW) directly.
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -39,6 +43,13 @@ struct AtArgs {
   const int *rows_a, *rows_b, *count;           // gather mode: [batch][pair_cap] row lists, [batch] K
   int pair_cap;
 };
+// conv mode: input / output maps and the kernel geometry.  A separate kernel parameter, so that the plain and gather instances
+// keep the AtArgs layout (and the code) they were built with
+struct AtConv {
+  int H, W, OH, OW, KW, stride, pad, dil;
+};
+
+enum { AT_PLAIN = 0, AT_GATHER = 1, AT_CONV = 2 };
 
 TT_DEVICE void split_rn(float x, float& hi, float& lo) {
   hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
@@ -47,8 +58,9 @@ TT_DEVICE void split_rn(float x, float& hi, float& lo) {
 TT_DEVICE void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> TT_DEVICE void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-template <bool GATHER>
-__global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p) {
+template <int MODE>
+__global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p, const AtConv cv) {
+  constexpr bool GATHER = MODE == AT_GATHER, CONV = MODE == AT_CONV;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* ops = smem;                                     // [2][A hi | A lo | B hi | B lo]
@@ -87,8 +99,16 @@ __global__ void __launch_bounds__(NT, 1) gemm_at_kernel(const AtArgs p) {
       const int c = tid + r * NT, kk = c >> 4, q = c & 15;
       const int k = k0 + kk, j = j0 + q * 4;
       const bool ok = k < K && j < p.N;
-      const long long row = GATHER ? (ok ? (long long)__ldg(rows_b + k) : 0) : k;
-      cp_async16(rb + c * 16, ok ? Bm + row * p.ldb + j : p.B, ok ? 16 : 0);
+      if constexpr (CONV) {                                // output pixel k -> the input pixel this tap reads, or zeros
+        const int kh = b / cv.KW, kw = b - kh * cv.KW;     // this batch's tap
+        const int ow = k % cv.OW, t2 = k / cv.OW, oh = t2 % cv.OH, n = t2 / cv.OH;
+        const int ih = oh * cv.stride - cv.pad + kh * cv.dil, iw = ow * cv.stride - cv.pad + kw * cv.dil;
+        const bool in = ok && ih >= 0 && ih < cv.H && iw >= 0 && iw < cv.W;
+        cp_async16(rb + c * 16, in ? p.B + (((long long)n * cv.H + ih) * cv.W + iw) * p.ldb + j : p.B, in ? 16 : 0);
+      } else {
+        const long long row = GATHER ? (ok ? (long long)__ldg(rows_b + k) : 0) : k;
+        cp_async16(rb + c * 16, ok ? Bm + row * p.ldb + j : p.B, ok ? 16 : 0);
+      }
     }
   };
   // staging stage s -> operand buffer o: transpose to K-major, split into hi / lo, 128-byte swizzle
@@ -232,9 +252,9 @@ int tt_gemm_at(const float* A, int lda, long long a_batch, const float* B, int l
   a.k_per = tt_cdiv(tt_cdiv(K, KS), a.splits);
   a.rows_a = a.rows_b = a.count = nullptr; a.pair_cap = 0;
   static bool set = false;
-  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<AT_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
   const long long items = (long long)batch * a.m_tiles * a.n_tiles * a.splits;
-  gemm_at_kernel<false><<<(unsigned)items, NT, SMEM, st>>>(a);
+  gemm_at_kernel<AT_PLAIN><<<(unsigned)items, NT, SMEM, st>>>(a, AtConv{});
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_gemm_at");
   const long long total = (long long)batch * M * N;
@@ -265,9 +285,9 @@ int tt_gemm_at_gather(const float* A, int lda, const int* rows_a, const float* B
   TT_REQUIRE(ws && ws_bytes >= (size_t)a.splits * batch * M * N * sizeof(float), "tt_gemm_at_gather",
              "workspace smaller than tt_gemm_at_workspace_bytes");
   static bool set = false;
-  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<AT_GATHER>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
   const long long items = (long long)batch * a.m_tiles * a.n_tiles * a.splits;
-  gemm_at_kernel<true><<<(unsigned)items, NT, SMEM, st>>>(a);
+  gemm_at_kernel<AT_GATHER><<<(unsigned)items, NT, SMEM, st>>>(a, AtConv{});
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_gemm_at_gather");
   const long long total = (long long)batch * M * N;
@@ -276,5 +296,55 @@ int tt_gemm_at_gather(const float* A, int lda, const int* rows_a, const float* B
                                                                                              c_batch, 0);
   ++g_tt_launches;
   TT_CHECK_LAUNCH("tt_gemm_at_gather(fold)");
+  return TT_OK;
+}
+
+// grad_weight (M, N, taps)[i][j][t] = part[0][t][i][j] + part[1][t][i][j] + ...  (in this order): torch's (Cout, Cin, KH, KW)
+static __global__ void gemm_at_fold_conv_kernel(const float* __restrict__ part, int splits, int taps, int M, int N, float* __restrict__ gw) {
+  const long long MN = (long long)M * N, total = taps * MN;
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int t = (int)(e % taps), j = (int)((e / taps) % N), i = (int)(e / ((long long)taps * N));
+    const long long src = (long long)t * MN + (long long)i * N + j;
+    float v = 0.f;
+    for (int s = 0; s < splits; ++s) v += part[s * total + src];
+    gw[e] = v;
+  }
+}
+
+// Conv form: gw[i][j][kh][kw] = sum over output pixels k < N*OH*OW of gy[k][i] * x(pixel k, tap (kh, kw))[j], gy [P][M] (row pitch M),
+// x [N][H][W][Cin = N cols] (row pitch Cin).  Same tiles, 3xTF32 products, fixed split count and fold order as tt_gemm_at (bitwise
+// reproducible); ws: tt_gemm_at_workspace_bytes(KH * KW, M, Cin).
+int tt_gemm_at_conv(const float* gy, const float* x, float* gw, int n_img, int H, int W, int OH, int OW, int KH, int KW, int stride, int pad,
+                    int dil, int M, int Cin, void* ws, size_t ws_bytes, cudaStream_t st) {
+  TT_REQUIRE(gy && x && gw, "tt_gemm_at_conv", "null argument");
+  TT_REQUIRE(M % 4 == 0 && Cin % 4 == 0 && ((reinterpret_cast<uintptr_t>(gy) | reinterpret_cast<uintptr_t>(x)) & 15) == 0, "tt_gemm_at_conv",
+             "M and Cin must be multiples of 4 floats, gy and x 16-byte aligned");
+  const int taps = KH * KW, K = n_img * OH * OW;
+  if (taps <= 0 || M <= 0 || Cin <= 0) return TT_OK;
+  if (K <= 0) {
+    if (cudaMemsetAsync(gw, 0, (size_t)taps * M * Cin * 4, st) != cudaSuccess) { tt_set_error("tt_gemm_at_conv: memset failed"); return TT_ERR_CUDA; }
+    return TT_OK;
+  }
+  AtArgs a;
+  a.A = gy; a.B = x; a.part = static_cast<float*>(ws);
+  a.M = M; a.N = Cin; a.K = K; a.lda = M; a.ldb = Cin; a.a_batch = a.b_batch = 0;
+  a.m_tiles = tt_cdiv(M, BM); a.n_tiles = tt_cdiv(Cin, BN); a.batch = taps;
+  a.splits = at_splits(taps, M, Cin, K);
+  a.k_per = tt_cdiv(tt_cdiv(K, KS), a.splits);
+  a.rows_a = a.rows_b = a.count = nullptr; a.pair_cap = 0;
+  const AtConv cv = {H, W, OH, OW, KW, stride, pad, dil};
+  TT_REQUIRE(ws && ws_bytes >= (size_t)a.splits * taps * M * Cin * sizeof(float), "tt_gemm_at_conv",
+             "workspace smaller than tt_gemm_at_workspace_bytes");
+  static bool set = false;
+  if (!set) { cudaFuncSetAttribute(gemm_at_kernel<AT_CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  const long long items = (long long)taps * a.m_tiles * a.n_tiles * a.splits;
+  gemm_at_kernel<AT_CONV><<<(unsigned)items, NT, SMEM, st>>>(a, cv);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH("tt_gemm_at_conv");
+  const long long total = (long long)taps * M * Cin;
+  const long long nb = (total + 255) / 256;
+  gemm_at_fold_conv_kernel<<<(int)(nb > tt_num_sms() * 8 ? tt_num_sms() * 8 : nb), 256, 0, st>>>(a.part, a.splits, taps, M, Cin, gw);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH("tt_gemm_at_conv(fold)");
   return TT_OK;
 }

@@ -65,6 +65,9 @@ struct TcArgs {
   // split-K (under-filled layers: few tiles, long K): work item = (tile, N tile, K split); partial sums are
   // red.add-ed into an output the host pre-initialised with bias + residuals, activation applied by a finish kernel
   int splits, k_per;     // K slabs per split (k_per * splits >= taps * n_slabs)
+  // input pixel of output (oh, ow) and tap (kh, kw): (oh * stride + org_h + kh * dil, ow * stride + org_w + kw * dil); -pad for a
+  // plain convolution, per dimension and of either sign for the stride phases of a transposed (input-gradient) convolution
+  int org_h, org_w;
 };
 constexpr int MAX_KVOL = 32;
 
@@ -204,7 +207,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         else {
           const int tw = mt % p.tiles_w, th = (mt / p.tiles_w) % p.tiles_h;
           cn = mt / (p.tiles_w * p.tiles_h);
-          cw0 = tw * p.TW * d.stride - d.pad; ch0 = th * p.TH * d.stride - d.pad;
+          cw0 = tw * p.TW * d.stride + p.org_w; ch0 = th * p.TH * d.stride + p.org_h;
         }
         for (int it = kb; it < ke; ++it, ++ig) {
           const int s = ig % STAGES;
@@ -471,8 +474,10 @@ extern "C" size_t tt_conv2d_workspace_bytes(const tt_conv_desc* d) {
 // w_tc: [2][Cout][taps][Cin] fp32 = TF32-exact hi plane then lo plane (prepared once per layer by the host).
 // allow_split_k = false keeps every output row's sum in one fixed order (no red.add across K splits): the deformable
 // convolution's outputs must not depend on how many images one call covers.
-int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const float* bias, const float* res,
-                 const float* res2, float* y, void* /*workspace*/, cudaStream_t st, bool allow_split_k) {
+// tt_conv2d_tc_origin: the same with the input origin given per dimension (org_h, org_w) instead of -pad (d->pad is not read),
+// and no shape predicate: OH / OW are whatever output extent the caller wants covered (input rows past the map read as zeros).
+int tt_conv2d_tc_origin(const tt_conv_desc* d, int org_h, int org_w, const float* x, const float* w_tc, const float* bias, const float* res,
+                        const float* res2, float* y, cudaStream_t st, bool allow_split_k) {
   const int terms = d->impl == 3 ? 3 : 1;
   const int taps = d->KH * d->KW;
   const long long npix_in = (long long)d->N * d->H * d->W;
@@ -485,7 +490,9 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
   a.chunk = terms == 3 ? ((g_tt_debug & 0x40000) ? 1 : (g_tt_debug & 0x20000) ? 4 : 2) : 16;   // 2 slabs = K 64: 8 truncating accumulations per chunk
   a.n_slabs = (d->Cin + KS - 1) / KS;
   a.total_pix = d->N * d->OH * d->OW;
-  a.flat = (taps == 1 && d->pad == 0 && d->stride == 1 && xhs == (long long)d->W * d->x_ld && xns == (long long)d->H * xhs) ? 1 : 0;
+  a.org_h = org_h; a.org_w = org_w;
+  a.flat = (taps == 1 && org_h == 0 && org_w == 0 && d->stride == 1 && d->OH == d->H && d->OW == d->W && xhs == (long long)d->W * d->x_ld &&
+            xns == (long long)d->H * xhs) ? 1 : 0;
   CUtensorMap ma, mb_hi, mb_lo;
   int grid_x;
   if (a.flat) {
@@ -568,6 +575,11 @@ int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const
     TT_CHECK_LAUNCH("tt_conv2d(tc split-k finish)");
   }
   return TT_OK;
+}
+
+int tt_conv2d_tc(const tt_conv_desc* d, const float* x, const float* w_tc, const float* bias, const float* res,
+                 const float* res2, float* y, void* /*workspace*/, cudaStream_t st, bool allow_split_k) {
+  return tt_conv2d_tc_origin(d, -d->pad, -d->pad, x, w_tc, bias, res, res2, y, st, allow_split_k);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -138,6 +138,11 @@ class CameraLossStats(C.Structure):
     _fields_ = [('ce', C.c_double), ('seg_factor', C.c_double), ('nseg', C.c_longlong), ('nfg', C.c_longlong), ('bad', C.c_longlong)]
 
 
+class Conv2dTrainDesc(C.Structure):
+    """tt_conv2d_train_desc (include/tt_b200.h section 16): shape and parameters of one training-side dense convolution."""
+    _fields_ = [(n, C.c_int) for n in ('N', 'H', 'W', 'Cin', 'Cout', 'KH', 'KW', 'stride', 'pad', 'dil', 'groups', 'bias', 'OH', 'OW')]
+
+
 _lib = None
 
 
@@ -155,7 +160,8 @@ def load():
     for n in ('tt_voxel_pooling_workspace_bytes', 'tt_lift_splat_workspace_bytes', 'tt_voxelize_workspace_bytes',
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
               'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes',
-              'tt_lift_splat_train_workspace_bytes', 'tt_loss_backward_workspace_bytes', 'tt_camera_loss_train_workspace_bytes'):
+              'tt_lift_splat_train_workspace_bytes', 'tt_loss_backward_workspace_bytes', 'tt_camera_loss_train_workspace_bytes',
+              'tt_conv2d_train_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -178,6 +184,7 @@ EXPORTS = [
     'tt_lift_splat_train_workspace_bytes', 'tt_lift_splat_train_forward', 'tt_lift_splat_train_backward',
     'tt_loss_backward_workspace_bytes', 'tt_loss_backward',
     'tt_camera_loss_train_workspace_bytes', 'tt_camera_loss_train_forward', 'tt_camera_loss_train_backward',
+    'tt_conv2d_train_workspace_bytes', 'tt_conv2d_train_forward', 'tt_conv2d_train_backward',
 ]
 
 
