@@ -3,7 +3,7 @@
  * ThinkTwice per-frame forward path.  It replaces `open_loop_training/ops` of the reference
  * (OpenDriveLab/ThinkTwice) and the third-party native ops the path crosses (mmcv._ext
  * ms_deform_attn / deform_conv / hard_voxelize, spconv, cuDNN/cuBLAS through torch.nn), and the training-side
- * gradients of the native ops, losses and dense convolutions on the reference's training step (sections 9, 10b and 12 to 16).
+ * gradients of the native ops, losses and dense convolutions on the reference's training step (sections 9, 10b and 12 to 17).
  *
  * Conventions (SURVEY.md §8b "External native ABIs"):
  *   - plain pointers and sizes only; every pointer is a DEVICE pointer unless it says "host";
@@ -673,6 +673,53 @@ int tt_conv2d_train_forward(const tt_conv2d_train_desc* d, const float* x, const
                             void* ws, size_t ws_bytes, tt_stream_t stream);
 int tt_conv2d_train_backward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* grad_y,
                              float* grad_x, float* grad_weight, float* grad_bias, void* ws, size_t ws_bytes, tt_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * (17) training-side upsampling: the UNet head's and the SECONDFPN deblock's torch.nn.ConvTranspose2d, and align_corners=True bilinear
+ * interpolation (nn.Upsample, the ASPP pooling branch's F.interpolate), forward and backward.  Conventions of section 16: activations
+ * and their gradients in torch's channels_last storage, fp32.
+ *
+ * Transposed convolution:
+ *   y[n][oh][ow][o] = bias[o] + sum over (i, kh, kw, h, w) with oh = h * stride - pad + kh, ow = w * stride - pad + kw of
+ *                     weight[i][o][kh][kw] x[n][h][w][i]
+ * x, grad_x [N][H][W][Cin]; y, grad_y [N][OH][OW][Cout]; weight, grad_weight torch's contiguous (Cin, Cout, KH, KW); bias, grad_bias
+ * [Cout].  This is the adjoint of the section 16 Conv2d with the same weight tensor (Cout_conv = Cin, Cin_conv = Cout, input OH x OW,
+ * output H x W), and it runs on that section's kernels: the forward is the Conv2d's per-phase grad_x path (the bias in its epilogue,
+ * and written into any phase no tap reaches), grad_x the Conv2d's forward, grad_weight its weight gradient with x and grad_y exchanged,
+ * grad_bias the column sums of grad_y.  3xTF32 products, fp32 accumulation; every output bitwise reproducible.
+ * Supported: groups 1, dil 1, stride 1 or 2, 0 <= output_padding < stride, pad >= 0, Cin and Cout multiples of 4, OH / OW equal to
+ * (H - 1) stride - 2 pad + KH + output_padding (resp. W, KW) and at least 1, counts within 32-bit indexing.  Anything else, and
+ * ws_bytes < tt_conv_transpose2d_train_workspace_bytes(d), returns TT_ERR_UNSUPPORTED with the parameter named in tt_last_error,
+ * before any pointer or device is touched.  N = 0 launches no kernel (grad_weight / grad_bias are zeroed by memset).
+ * Forward: y is fully written; bias is read when d->bias (NULL otherwise).  Backward: grad_x, grad_weight and grad_bias (when d->bias)
+ * are fully written; any of them may be NULL and is then not computed.
+ * ws: tt_conv_transpose2d_train_workspace_bytes(d) bytes of device memory, not shared with a concurrent call.
+ *
+ * Bilinear interpolation, align_corners = True (the only mode the model uses; 0 is refused): x, grad_x [N][H][W][C]; y, grad_y
+ * [N][OH][OW][C], any OH, OW >= 1 (x2 upsampling, and the 1 x 1 -> OH x OW broadcast).  The forward is ATen's CUDA arithmetic:
+ * scale_h = OH > 1 ? (float)(H - 1) / (OH - 1) : 0, source row r = scale_h * oh, h0 = (int)r, h1 = h0 + (h0 < H - 1), l = r - h0,
+ *   y = (1 - l_h) ((1 - l_w) x[h0][w0] + l_w x[h0][w1]) + l_h ((1 - l_w) x[h1][w0] + l_w x[h1][w1]).
+ * The backward is a gather, no atomics: each input pixel sums, in a fixed order, the output pixels that read it (along each
+ * dimension a contiguous range of output rows), so grad_x is fully written and bitwise reproducible.  An input pixel that many output
+ * pixels reach (the broadcast) is summed by several row lanes folded in lane order.
+ * Refused with TT_ERR_UNSUPPORTED, the parameter named: align_corners != 1, C not a positive multiple of 4, N < 0, H / W / OH / OW < 1,
+ * counts past 32-bit indexing.  N = 0 launches nothing.  x, y, grad_y, grad_x 16-byte aligned.
+ */
+typedef struct {
+  int N, H, W, Cin, Cout, KH, KW, stride, pad, output_padding, dil, groups, bias;
+  int OH, OW;
+} tt_conv_transpose2d_train_desc;
+size_t tt_conv_transpose2d_train_workspace_bytes(const tt_conv_transpose2d_train_desc* d);   /* 0 when refused */
+int tt_conv_transpose2d_train_forward(const tt_conv_transpose2d_train_desc* d, const float* x, const float* weight, const float* bias,
+                                      float* y, void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_conv_transpose2d_train_backward(const tt_conv_transpose2d_train_desc* d, const float* x, const float* weight, const float* grad_y,
+                                       float* grad_x, float* grad_weight, float* grad_bias, void* ws, size_t ws_bytes, tt_stream_t stream);
+
+typedef struct {
+  int N, C, H, W, OH, OW, align_corners;
+} tt_interp_bilinear_train_desc;
+int tt_interp_bilinear_train_forward(const tt_interp_bilinear_train_desc* d, const float* x, float* y, tt_stream_t stream);
+int tt_interp_bilinear_train_backward(const tt_interp_bilinear_train_desc* d, const float* grad_y, float* grad_x, tt_stream_t stream);
 
 #ifdef __cplusplus
 }

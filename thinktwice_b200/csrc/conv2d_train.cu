@@ -13,6 +13,14 @@
 //                its plain mode), split over pixels and folded in a fixed order;
 //   grad_bias  : per-channel column sums of grad_y over fixed row chunks, folded in chunk order.
 // No floating-point atomics and no red.add split-K anywhere: every output is bitwise reproducible.
+//
+// Training-side transposed convolution (torch.nn.ConvTranspose2d, groups 1, dilation 1): its (Cin, Cout, KH, KW) weight is exactly the
+// weight of the adjoint Conv2d (Cout_conv = Cin, Cin_conv = Cout) whose input is the transposed output, so it runs on the same kernels:
+//   forward    : the adjoint's grad_x path with x in the role of grad_y, the bias in the phase convolutions' epilogue (and written into
+//                any phase no tap reaches);
+//   grad_x     : the adjoint's forward applied to grad_y, no bias;
+//   grad_weight: the adjoint's weight gradient with x := grad_y and grad_y := x;
+//   grad_bias  : the column sums of grad_y.
 #include "common.cuh"
 
 extern long long g_tt_launches;
@@ -100,14 +108,16 @@ __global__ void c2t_pack_weight_kernel(const float* __restrict__ w, float* __res
   }
 }
 
-// grad_x pixels of the phases in `mask` (bit py * s + px) no tap reaches: zeros
-__global__ void c2t_zero_phases_kernel(float* __restrict__ gx, int N, int H, int W, int C, int s, int mask) {
+// grad_x pixels of the phases in `mask` (bit py * s + px) no tap reaches: zeros, or the bias (kBias, the transposed forward)
+template <bool kBias>
+__global__ void c2t_fill_phases_kernel(float* __restrict__ gx, int N, int H, int W, int C, int s, int mask, const float* __restrict__ bias) {
   const int C4 = C / 4;
   const long long total = (long long)N * H * W * C4;
   for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const long long pix = e / C4;
     const int w = (int)(pix % W), h = (int)((pix / W) % H);
-    if (mask >> ((h % s) * s + (w % s)) & 1) reinterpret_cast<float4*>(gx)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (mask >> ((h % s) * s + (w % s)) & 1)
+      reinterpret_cast<float4*>(gx)[e] = kBias ? __ldg(reinterpret_cast<const float4*>(bias) + e % C4) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 
@@ -150,15 +160,15 @@ int bias_chunks(long long P) {
   return (int)(c < 1 ? 1 : c > BIAS_CHUNKS ? BIAS_CHUNKS : c);
 }
 
-// the workspace of one call, carved in 256-byte aligned pieces
+// the workspace of one call, carved in 256-byte aligned pieces; grad_bias sums bias_c columns (d->Cout; a transposed conv's d->Cin)
 struct Ws {
   float *wf, *wb, *part, *bpart;
   size_t part_bytes, bytes;
 };
-Ws carve(const tt_conv2d_train_desc* d, void* base) {
+Ws carve(const tt_conv2d_train_desc* d, void* base, int bias_c) {
   const long long wsz = (long long)d->Cout * d->Cin * d->KH * d->KW;
   const size_t part = tt_gemm_at_workspace_bytes(d->KH * d->KW, d->Cout, d->Cin);
-  const size_t sizes[4] = {(size_t)2 * wsz * 4, (size_t)2 * wsz * 4, part, (size_t)BIAS_CHUNKS * d->Cout * 4};
+  const size_t sizes[4] = {(size_t)2 * wsz * 4, (size_t)2 * wsz * 4, part, (size_t)BIAS_CHUNKS * bias_c * 4};
   Ws w;
   float** slots[4] = {&w.wf, &w.wb, &w.part, &w.bpart};
   size_t o = 0;
@@ -202,9 +212,9 @@ int check_desc(const tt_conv2d_train_desc* d, const char* name) {
   return TT_OK;
 }
 
-int check_ws(const tt_conv2d_train_desc* d, size_t ws_bytes, const char* name) {
-  if (ws_bytes < carve(d, nullptr).bytes) {
-    tt_set_error("%s: unsupported ws_bytes: smaller than tt_conv2d_train_workspace_bytes", name);
+int check_ws(const tt_conv2d_train_desc* d, int bias_c, size_t ws_bytes, const char* name, const char* ws_fn) {
+  if (ws_bytes < carve(d, nullptr, bias_c).bytes) {
+    tt_set_error("%s: unsupported ws_bytes: smaller than %s", name, ws_fn);
     return TT_ERR_UNSUPPORTED;
   }
   return TT_OK;
@@ -227,94 +237,184 @@ tt_conv_desc tc_desc(int N, int H, int W, int Cin, int Cout, int KH, int KW, int
     if (rc__ != TT_OK) return rc__;      \
   } while (0)
 
-}  // namespace
-
-extern "C" size_t tt_conv2d_train_workspace_bytes(const tt_conv2d_train_desc* d) {
-  if (check_desc(d, "tt_conv2d_train_workspace_bytes") != TT_OK) return 0;
-  return carve(d, nullptr).bytes;
-}
-
-extern "C" int tt_conv2d_train_forward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* bias, float* y,
-                                       void* ws, size_t ws_bytes, tt_stream_t stream) {
-  static const char* name = "tt_conv2d_train_forward";
-  C2T_CALL(check_desc(d, name));
-  C2T_CALL(check_ws(d, ws_bytes, name));
-  if (d->N == 0) return TT_OK;
-  TT_REQUIRE(x && weight && y && ws && (bias || !d->bias), name, "null argument");
-  TT_REQUIRE(aligned16(x) && aligned16(y) && aligned16(ws) && (!bias || aligned16(bias)), name, "x, y, bias and ws must be 16-byte aligned");
-  cudaStream_t st = (cudaStream_t)stream;
-  const Ws w = carve(d, ws);
+// y = conv2d(x, weight) (+ bias when non-NULL): the weight packed into w.wf, then the implicit-GEMM convolution
+int c2t_conv(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* bias, float* y, const Ws& w, cudaStream_t st,
+             const char* name) {
   const Phases P = make_phases(d);
   c2t_pack_weight_kernel<<<grid_for((long long)d->Cout * d->Cin * d->KH * d->KW, 256), 256, 0, st>>>(weight, w.wf, nullptr, d->Cout, d->Cin,
                                                                                                        d->KH, d->KW, d->pad, d->dil, P);
   ++g_tt_launches;
   TT_CHECK_LAUNCH(name);
   const tt_conv_desc c = tc_desc(d->N, d->H, d->W, d->Cin, d->Cout, d->KH, d->KW, d->stride, d->pad, d->dil, d->OH, d->OW);
-  return tt_conv2d_tc(&c, x, w.wf, d->bias ? bias : nullptr, nullptr, nullptr, y, nullptr, st, false);
+  return tt_conv2d_tc(&c, x, w.wf, bias, nullptr, nullptr, y, nullptr, st, false);
+}
+
+// gx [N][H][W][Cin] = the input gradient of conv2d from gy [N][OH][OW][Cout] (+ bias [Cin] on every pixel when non-NULL): one stride-1
+// convolution per output phase, stored through the pixel scatter; phases no tap reaches get zeros (or the bias)
+int c2t_phase_conv(const tt_conv2d_train_desc* d, const float* weight, const float* gy, const float* bias, float* gx, const Ws& w,
+                   cudaStream_t st, const char* name) {
+  const Phases ph = make_phases(d);
+  c2t_pack_weight_kernel<<<grid_for((long long)d->Cout * d->Cin * d->KH * d->KW, 256), 256, 0, st>>>(weight, nullptr, w.wb, d->Cout, d->Cin,
+                                                                                                       d->KH, d->KW, d->pad, d->dil, ph);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH(name);
+  int empty = 0;
+  for (int q = 0; q < ph.s * ph.s; ++q) {
+    const Dim& dh = ph.h[q / ph.s];
+    const Dim& dw = ph.w[q % ph.s];
+    if (dh.ext == 0 || dw.ext == 0) continue;                 // no grad_x pixel in this phase
+    if (dh.n == 0 || dw.n == 0) { empty |= 1 << q; continue; }
+    tt_conv_desc c = tc_desc(d->N, d->OH, d->OW, d->Cout, d->Cin, dh.n, dw.n, 1, 0, ph.dil, dh.ext, dw.ext);
+    c.yH = d->H; c.yW = d->W;
+    c.oy_mul = c.ox_mul = ph.s; c.oy_add = q / ph.s; c.ox_add = q % ph.s;
+    C2T_CALL(tt_conv2d_tc_origin(&c, dh.org, dw.org, gy, w.wb + ph.off[q], bias, nullptr, nullptr, gx, st, false));
+  }
+  if (empty) {
+    const int nb = grid_for((long long)d->N * d->H * d->W * (d->Cin / 4), 256);
+    if (bias) c2t_fill_phases_kernel<true><<<nb, 256, 0, st>>>(gx, d->N, d->H, d->W, d->Cin, ph.s, empty, bias);
+    else c2t_fill_phases_kernel<false><<<nb, 256, 0, st>>>(gx, d->N, d->H, d->W, d->Cin, ph.s, empty, nullptr);
+    ++g_tt_launches;
+    TT_CHECK_LAUNCH(name);
+  }
+  return TT_OK;
+}
+
+// gw [Cout][Cin][KH][KW] = the weight gradient of conv2d from x [N][H][W][Cin] and gy [N][OH][OW][Cout]
+int c2t_weight_grad(const tt_conv2d_train_desc* d, const float* x, const float* gy, float* gw, const Ws& w, cudaStream_t st) {
+  if (d->KH == 1 && d->KW == 1 && d->stride == 1 && d->pad == 0)   // pixel k of grad_y meets pixel k of x: the plain contraction
+    return tt_gemm_at(gy, d->Cout, 0, x, d->Cin, 0, gw, d->Cin, 0, 1, d->Cout, d->Cin, (int)((long long)d->N * d->OH * d->OW), 0, w.part,
+                      w.part_bytes, st);
+  return tt_gemm_at_conv(gy, x, gw, d->N, d->H, d->W, d->OH, d->OW, d->KH, d->KW, d->stride, d->pad, d->dil, d->Cout, d->Cin, w.part,
+                         w.part_bytes, st);
+}
+
+// gb [C] = per-column sums of g [P][C] over fixed row chunks, folded in chunk order
+int c2t_bias_sum(const float* g, long long P, int C, float* gb, const Ws& w, cudaStream_t st, const char* name) {
+  const int chunks = bias_chunks(P), rows_per = (int)((P + chunks - 1) / chunks);
+  c2t_bias_part_kernel<<<dim3(tt_cdiv(C, 128), chunks), 256, 0, st>>>(g, (int)P, C, rows_per, w.bpart);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH(name);
+  c2t_bias_fold_kernel<<<tt_cdiv(C, 256), 256, 0, st>>>(w.bpart, chunks, C, gb);
+  ++g_tt_launches;
+  TT_CHECK_LAUNCH(name);
+  return TT_OK;
+}
+
+// an empty batch: zero parameter gradients, no kernel
+int zero_params(float* gw, long long wsz, float* gb, int bias_c, cudaStream_t st, const char* name) {
+  if ((gw && cudaMemsetAsync(gw, 0, (size_t)wsz * 4, st) != cudaSuccess) || (gb && cudaMemsetAsync(gb, 0, (size_t)bias_c * 4, st) != cudaSuccess)) {
+    tt_set_error("%s: memset failed", name);
+    return TT_ERR_CUDA;
+  }
+  return TT_OK;
+}
+
+// the transposed convolution t as its adjoint Conv2d d (the same weight tensor, Cin and Cout exchanged, H / W the transposed output);
+// refuses what the library does not build, naming the transposed parameter; touches no pointer and no device
+int adjoint_desc(const tt_conv_transpose2d_train_desc* t, tt_conv2d_train_desc* d, const char* name) {
+  if (!t) {
+    tt_set_error("%s: null descriptor", name);
+    return TT_ERR_INVALID;
+  }
+  const char* bad = nullptr;
+  const long long oh = ((long long)t->H - 1) * t->stride - 2LL * t->pad + t->KH + t->output_padding;
+  const long long ow = ((long long)t->W - 1) * t->stride - 2LL * t->pad + t->KW + t->output_padding;
+  if (t->groups != 1) bad = "groups: only 1 is supported";
+  else if (t->dil != 1) bad = "dil: only 1 is supported";
+  else if (t->stride != 1 && t->stride != 2) bad = "stride: only 1 and 2 are supported";
+  else if (t->output_padding < 0 || t->output_padding >= t->stride) bad = "output_padding: must be >= 0 and < stride";
+  else if (t->Cin <= 0 || t->Cin % 4) bad = "Cin: must be a positive multiple of 4";
+  else if (t->Cout <= 0 || t->Cout % 4) bad = "Cout: must be a positive multiple of 4";
+  else if (t->KH < 1 || t->KW < 1) bad = "KH / KW: must be >= 1";
+  else if (t->pad < 0) bad = "pad: must be >= 0";
+  else if (t->bias != 0 && t->bias != 1) bad = "bias: must be 0 or 1";
+  else if (t->N < 0 || t->H < 1 || t->W < 1) bad = "N / H / W: N must be >= 0, H and W >= 1";
+  else if (t->OH != oh || oh < 1) bad = "OH: does not match (H - 1) stride - 2 pad + KH + output_padding";
+  else if (t->OW != ow || ow < 1) bad = "OW: does not match (W - 1) stride - 2 pad + KW + output_padding";
+  if (bad) {
+    tt_set_error("%s: unsupported %s", name, bad);
+    return TT_ERR_UNSUPPORTED;
+  }
+  *d = tt_conv2d_train_desc{t->N, t->OH, t->OW, t->Cout, t->Cin, t->KH, t->KW, t->stride, t->pad, 1, 1, t->bias, t->H, t->W};
+  return check_desc(d, name);   // what is left to refuse: counts past 32-bit indexing
+}
+
+}  // namespace
+
+extern "C" size_t tt_conv2d_train_workspace_bytes(const tt_conv2d_train_desc* d) {
+  if (check_desc(d, "tt_conv2d_train_workspace_bytes") != TT_OK) return 0;
+  return carve(d, nullptr, d->Cout).bytes;
+}
+
+extern "C" int tt_conv2d_train_forward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* bias, float* y,
+                                       void* ws, size_t ws_bytes, tt_stream_t stream) {
+  static const char* name = "tt_conv2d_train_forward";
+  C2T_CALL(check_desc(d, name));
+  C2T_CALL(check_ws(d, d->Cout, ws_bytes, name, "tt_conv2d_train_workspace_bytes"));
+  if (d->N == 0) return TT_OK;
+  TT_REQUIRE(x && weight && y && ws && (bias || !d->bias), name, "null argument");
+  TT_REQUIRE(aligned16(x) && aligned16(y) && aligned16(ws) && (!bias || aligned16(bias)), name, "x, y, bias and ws must be 16-byte aligned");
+  return c2t_conv(d, x, weight, d->bias ? bias : nullptr, y, carve(d, ws, d->Cout), (cudaStream_t)stream, name);
 }
 
 extern "C" int tt_conv2d_train_backward(const tt_conv2d_train_desc* d, const float* x, const float* weight, const float* grad_y,
                                         float* grad_x, float* grad_weight, float* grad_bias, void* ws, size_t ws_bytes, tt_stream_t stream) {
   static const char* name = "tt_conv2d_train_backward";
   C2T_CALL(check_desc(d, name));
-  C2T_CALL(check_ws(d, ws_bytes, name));
+  C2T_CALL(check_ws(d, d->Cout, ws_bytes, name, "tt_conv2d_train_workspace_bytes"));
   if (!d->bias) grad_bias = nullptr;
   if (!grad_x && !grad_weight && !grad_bias) return TT_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const long long wsz = (long long)d->Cout * d->Cin * d->KH * d->KW;
-  if (d->N == 0) {   // an empty batch: zero gradients, no kernel
-    if ((grad_weight && cudaMemsetAsync(grad_weight, 0, (size_t)wsz * 4, st) != cudaSuccess) ||
-        (grad_bias && cudaMemsetAsync(grad_bias, 0, (size_t)d->Cout * 4, st) != cudaSuccess)) {
-      tt_set_error("%s: memset failed", name);
-      return TT_ERR_CUDA;
-    }
-    return TT_OK;
-  }
+  if (d->N == 0) return zero_params(grad_weight, (long long)d->Cout * d->Cin * d->KH * d->KW, grad_bias, d->Cout, st, name);
   TT_REQUIRE(grad_y && ws && (!grad_x || weight) && (!grad_weight || x), name, "null argument");
   TT_REQUIRE(aligned16(grad_y) && aligned16(ws) && (!grad_x || aligned16(grad_x)) && (!grad_weight || aligned16(x)) &&
                  (!grad_bias || aligned16(grad_bias)),
              name, "x, grad_y, grad_x, grad_bias and ws must be 16-byte aligned");
-  const Ws w = carve(d, ws);
-  const long long P = (long long)d->N * d->OH * d->OW;
-  if (grad_x) {
-    const Phases ph = make_phases(d);
-    c2t_pack_weight_kernel<<<grid_for(wsz, 256), 256, 0, st>>>(weight, nullptr, w.wb, d->Cout, d->Cin, d->KH, d->KW, d->pad, d->dil, ph);
-    ++g_tt_launches;
-    TT_CHECK_LAUNCH(name);
-    int empty = 0;
-    for (int q = 0; q < ph.s * ph.s; ++q) {
-      const Dim& dh = ph.h[q / ph.s];
-      const Dim& dw = ph.w[q % ph.s];
-      if (dh.ext == 0 || dw.ext == 0) continue;                 // no grad_x pixel in this phase
-      if (dh.n == 0 || dw.n == 0) { empty |= 1 << q; continue; }
-      tt_conv_desc c = tc_desc(d->N, d->OH, d->OW, d->Cout, d->Cin, dh.n, dw.n, 1, 0, ph.dil, dh.ext, dw.ext);
-      c.yH = d->H; c.yW = d->W;
-      c.oy_mul = c.ox_mul = ph.s; c.oy_add = q / ph.s; c.ox_add = q % ph.s;
-      C2T_CALL(tt_conv2d_tc_origin(&c, dh.org, dw.org, grad_y, w.wb + ph.off[q], nullptr, nullptr, nullptr, grad_x, st, false));
-    }
-    if (empty) {
-      c2t_zero_phases_kernel<<<grid_for((long long)d->N * d->H * d->W * (d->Cin / 4), 256), 256, 0, st>>>(grad_x, d->N, d->H, d->W, d->Cin,
-                                                                                                          ph.s, empty);
-      ++g_tt_launches;
-      TT_CHECK_LAUNCH(name);
-    }
-  }
-  if (grad_weight) {
-    if (d->KH == 1 && d->KW == 1 && d->stride == 1 && d->pad == 0) {   // pixel k of grad_y meets pixel k of x: the plain contraction
-      C2T_CALL(tt_gemm_at(grad_y, d->Cout, 0, x, d->Cin, 0, grad_weight, d->Cin, 0, 1, d->Cout, d->Cin, (int)P, 0, w.part, w.part_bytes, st));
-    } else {
-      C2T_CALL(tt_gemm_at_conv(grad_y, x, grad_weight, d->N, d->H, d->W, d->OH, d->OW, d->KH, d->KW, d->stride, d->pad, d->dil, d->Cout,
-                               d->Cin, w.part, w.part_bytes, st));
-    }
-  }
-  if (grad_bias) {
-    const int chunks = bias_chunks(P), rows_per = (int)((P + chunks - 1) / chunks);
-    c2t_bias_part_kernel<<<dim3(tt_cdiv(d->Cout, 128), chunks), 256, 0, st>>>(grad_y, (int)P, d->Cout, rows_per, w.bpart);
-    ++g_tt_launches;
-    TT_CHECK_LAUNCH(name);
-    c2t_bias_fold_kernel<<<tt_cdiv(d->Cout, 256), 256, 0, st>>>(w.bpart, chunks, d->Cout, grad_bias);
-    ++g_tt_launches;
-    TT_CHECK_LAUNCH(name);
-  }
+  const Ws w = carve(d, ws, d->Cout);
+  if (grad_x) C2T_CALL(c2t_phase_conv(d, weight, grad_y, nullptr, grad_x, w, st, name));
+  if (grad_weight) C2T_CALL(c2t_weight_grad(d, x, grad_y, grad_weight, w, st));
+  if (grad_bias) C2T_CALL(c2t_bias_sum(grad_y, (long long)d->N * d->OH * d->OW, d->Cout, grad_bias, w, st, name));
+  return TT_OK;
+}
+
+// The transposed convolution is the adjoint of the Conv2d d that adjoint_desc builds: its forward is d's input gradient (plus the bias),
+// its input gradient d's forward, its weight gradient d's weight gradient with the roles of x and grad_y exchanged.
+extern "C" size_t tt_conv_transpose2d_train_workspace_bytes(const tt_conv_transpose2d_train_desc* t) {
+  tt_conv2d_train_desc d;
+  if (adjoint_desc(t, &d, "tt_conv_transpose2d_train_workspace_bytes") != TT_OK) return 0;
+  return carve(&d, nullptr, t->Cout).bytes;
+}
+
+extern "C" int tt_conv_transpose2d_train_forward(const tt_conv_transpose2d_train_desc* t, const float* x, const float* weight, const float* bias,
+                                                 float* y, void* ws, size_t ws_bytes, tt_stream_t stream) {
+  static const char* name = "tt_conv_transpose2d_train_forward";
+  tt_conv2d_train_desc d;
+  C2T_CALL(adjoint_desc(t, &d, name));
+  C2T_CALL(check_ws(&d, t->Cout, ws_bytes, name, "tt_conv_transpose2d_train_workspace_bytes"));
+  if (t->N == 0) return TT_OK;
+  TT_REQUIRE(x && weight && y && ws && (bias || !t->bias), name, "null argument");
+  TT_REQUIRE(aligned16(x) && aligned16(y) && aligned16(ws) && (!bias || aligned16(bias)), name, "x, y, bias and ws must be 16-byte aligned");
+  return c2t_phase_conv(&d, weight, x, t->bias ? bias : nullptr, y, carve(&d, ws, t->Cout), (cudaStream_t)stream, name);
+}
+
+extern "C" int tt_conv_transpose2d_train_backward(const tt_conv_transpose2d_train_desc* t, const float* x, const float* weight,
+                                                  const float* grad_y, float* grad_x, float* grad_weight, float* grad_bias, void* ws,
+                                                  size_t ws_bytes, tt_stream_t stream) {
+  static const char* name = "tt_conv_transpose2d_train_backward";
+  tt_conv2d_train_desc d;
+  C2T_CALL(adjoint_desc(t, &d, name));
+  C2T_CALL(check_ws(&d, t->Cout, ws_bytes, name, "tt_conv_transpose2d_train_workspace_bytes"));
+  if (!t->bias) grad_bias = nullptr;
+  if (!grad_x && !grad_weight && !grad_bias) return TT_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (t->N == 0) return zero_params(grad_weight, (long long)t->Cin * t->Cout * t->KH * t->KW, grad_bias, t->Cout, st, name);
+  TT_REQUIRE(grad_y && ws && (!grad_x || weight) && (!grad_weight || x), name, "null argument");
+  TT_REQUIRE(aligned16(grad_y) && aligned16(ws) && (!grad_x || aligned16(grad_x)) && (!grad_weight || aligned16(x)) &&
+                 (!grad_bias || aligned16(grad_bias)),
+             name, "x, grad_y, grad_x, grad_bias and ws must be 16-byte aligned");
+  const Ws w = carve(&d, ws, t->Cout);
+  if (grad_x) C2T_CALL(c2t_conv(&d, grad_y, weight, nullptr, grad_x, w, st, name));
+  if (grad_weight) C2T_CALL(c2t_weight_grad(&d, grad_y, x, grad_weight, w, st));
+  if (grad_bias) C2T_CALL(c2t_bias_sum(grad_y, (long long)t->N * t->OH * t->OW, t->Cout, grad_bias, w, st, name));
   return TT_OK;
 }

@@ -143,6 +143,17 @@ class Conv2dTrainDesc(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('N', 'H', 'W', 'Cin', 'Cout', 'KH', 'KW', 'stride', 'pad', 'dil', 'groups', 'bias', 'OH', 'OW')]
 
 
+class ConvTranspose2dTrainDesc(C.Structure):
+    """tt_conv_transpose2d_train_desc (include/tt_b200.h section 17): shape and parameters of one training-side transposed convolution."""
+    _fields_ = [(n, C.c_int) for n in ('N', 'H', 'W', 'Cin', 'Cout', 'KH', 'KW', 'stride', 'pad', 'output_padding', 'dil', 'groups', 'bias',
+                                        'OH', 'OW')]
+
+
+class InterpBilinearTrainDesc(C.Structure):
+    """tt_interp_bilinear_train_desc (include/tt_b200.h section 17): shapes of one align_corners bilinear interpolation."""
+    _fields_ = [(n, C.c_int) for n in ('N', 'C', 'H', 'W', 'OH', 'OW', 'align_corners')]
+
+
 _lib = None
 
 
@@ -161,7 +172,7 @@ def load():
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
               'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes',
               'tt_lift_splat_train_workspace_bytes', 'tt_loss_backward_workspace_bytes', 'tt_camera_loss_train_workspace_bytes',
-              'tt_conv2d_train_workspace_bytes'):
+              'tt_conv2d_train_workspace_bytes', 'tt_conv_transpose2d_train_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -185,6 +196,8 @@ EXPORTS = [
     'tt_loss_backward_workspace_bytes', 'tt_loss_backward',
     'tt_camera_loss_train_workspace_bytes', 'tt_camera_loss_train_forward', 'tt_camera_loss_train_backward',
     'tt_conv2d_train_workspace_bytes', 'tt_conv2d_train_forward', 'tt_conv2d_train_backward',
+    'tt_conv_transpose2d_train_workspace_bytes', 'tt_conv_transpose2d_train_forward', 'tt_conv_transpose2d_train_backward',
+    'tt_interp_bilinear_train_forward', 'tt_interp_bilinear_train_backward',
 ]
 
 

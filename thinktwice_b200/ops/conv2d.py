@@ -142,6 +142,12 @@ def convert_conv2d(module, prefix=''):
         new.train(m.training)
         return new
 
+    return swap_modules(module, prefix, swap), skipped
+
+
+def swap_modules(module, prefix, swap):
+    """Replace `module` (itself included) and its descendants by swap(m, qualified name), which returns m to keep it; the children of a
+    replaced module are not visited.  Returns the (possibly replaced) root."""
     def walk(m, name):
         for child_name, child in list(m.named_children()):
             full = f'{name}.{child_name}' if name else child_name
@@ -154,4 +160,4 @@ def convert_conv2d(module, prefix=''):
     root = swap(module, prefix)
     if root is module:
         walk(module, prefix)
-    return root, skipped
+    return root
