@@ -721,6 +721,59 @@ typedef struct {
 int tt_interp_bilinear_train_forward(const tt_interp_bilinear_train_desc* d, const float* x, float* y, tt_stream_t stream);
 int tt_interp_bilinear_train_backward(const tt_interp_bilinear_train_desc* d, const float* grad_y, float* grad_x, tt_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------
+ * (18) training-side batch normalization: torch.nn.BatchNorm1d / BatchNorm2d / SyncBatchNorm with batch statistics, forward and
+ * backward, with an optional residual and ReLU fused.  Operands are rows, C contiguous: x, r, y, grad_y, grad_x, grad_r [M][C] fp32
+ * (BatchNorm2d on channels_last, M = N H W; BatchNorm1d on (N, C); the sparse encoder's (sites, C) features); weight, bias,
+ * running_mean, running_var, grad_weight, grad_bias [C].  With mean and invstd per channel:
+ *   xhat = (x - mean) * invstd,   z = weight * xhat + bias (+ r),   y = act(z)   (act: TT_ACT_NONE or TT_ACT_RELU, y = z <= 0 ? 0 : z)
+ * in fp32, in that order, by one device function the forward and both backward passes share (the backward's ReLU mask is the
+ * forward's bit for bit; no mask and no y is kept).  A synchronized layer runs on R ranks; the collectives sit between the calls, in
+ * the caller, and this library calls no communication library.  Per layer, in order:
+ *   1. tt_batch_norm_train_stats: this rank's record[3][C] doubles, planar: record[0][c] = count (rows), record[1][c] = mean,
+ *      record[2][c] = M2 (sum of squared deviations), in fp64, over fixed row chunks (of a shifted sum each) folded by Chan's formula in
+ *      a fixed order.  M = 0 writes count 0, mean 0, M2 0.
+ *   2. tt_batch_norm_train_fold: records[R][3][C] (the R ranks' records in rank order; R = 1 unsynchronized) folded in rank order by
+ *      Chan's formula in fp64 -> mean[c] and invstd[c] = 1 / sqrt(M2 / n + eps) (fp32, for the passes below), and the running update
+ *      running = (1 - factor) running + factor stat with the unbiased variance M2 / (n - 1), as torch does.  n = the global count.
+ *   3. tt_batch_norm_train_forward: one pass reading x (and r), writing y.
+ *   4. tt_batch_norm_train_backward_reduce: one pass over x, r and grad_y; dz = grad_y masked by the recomputed z; writes this rank's
+ *      record[2][C] doubles: record[0][c] = sum dz, record[1][c] = sum dz xhat (fp64, fixed row chunks folded in a fixed order), and
+ *      from these LOCAL sums grad_bias = sum dz and grad_weight = sum dz xhat (torch's SyncBatchNorm leaves the parameter gradients
+ *      per rank for the data-parallel wrapper to average).
+ *   5. tt_batch_norm_train_backward: folds records[R][2][C] in rank order and writes grad_x = weight invstd (dz - sum dz / n - xhat sum
+ *      dz xhat / n), n = d->count, and grad_r = dz when d->residual.
+ * With d->training = 0 (eval mode) the forward and both backward passes take running_mean and running_var in the mean / invstd
+ * slots, with invstd = 1 / sqrtf(running_var + eps) per channel; then grad_x = weight invstd dz and records are not read.
+ * Every output is bitwise reproducible for a fixed split of the rows over ranks (the split changes only the fold); no floating-point
+ * atomics.  Any of grad_x, grad_r, grad_weight, grad_bias may be NULL and is then not computed; record is always written.
+ * Supported: affine 1, track_running_stats 1, C a positive multiple of 4, M >= 0, R >= 1, eps > 0, act TT_ACT_NONE / TT_ACT_RELU,
+ * residual and training 0 / 1, (backward, training) count >= 1.  Anything else, and ws_bytes < tt_batch_norm_train_workspace_bytes(d),
+ * returns TT_ERR_UNSUPPORTED with the parameter named in tt_last_error, before any pointer is touched.  M = 0 launches no pass over
+ * rows.  Row operands 16-byte aligned.  ws: not shared with a concurrent call.
+ */
+typedef struct {
+  long long M;                  /* rows of this rank */
+  long long count;              /* global rows n over the R ranks (tt_batch_norm_train_backward) */
+  int C, R;
+  int affine, track_running_stats, training, residual, act;
+  double eps;
+  double factor;                /* running-stat factor: momentum, or 1 / num_batches_tracked when momentum is None */
+} tt_batch_norm_train_desc;
+size_t tt_batch_norm_train_workspace_bytes(const tt_batch_norm_train_desc* d);   /* 0 when refused */
+int tt_batch_norm_train_stats(const tt_batch_norm_train_desc* d, const float* x, double* record, void* ws, size_t ws_bytes,
+                              tt_stream_t stream);
+int tt_batch_norm_train_fold(const tt_batch_norm_train_desc* d, const double* records, float* running_mean, float* running_var,
+                             float* mean, float* invstd, tt_stream_t stream);
+int tt_batch_norm_train_forward(const tt_batch_norm_train_desc* d, const float* x, const float* r, const float* weight, const float* bias,
+                                const float* mean, const float* invstd, float* y, tt_stream_t stream);
+int tt_batch_norm_train_backward_reduce(const tt_batch_norm_train_desc* d, const float* x, const float* r, const float* weight,
+                                        const float* bias, const float* mean, const float* invstd, const float* grad_y, double* record,
+                                        float* grad_weight, float* grad_bias, void* ws, size_t ws_bytes, tt_stream_t stream);
+int tt_batch_norm_train_backward(const tt_batch_norm_train_desc* d, const float* x, const float* r, const float* weight, const float* bias,
+                                 const float* mean, const float* invstd, const float* grad_y, const double* records, float* grad_x,
+                                 float* grad_r, tt_stream_t stream);
+
 #ifdef __cplusplus
 }
 /* C++ linkage, mangled exactly like the reference's own definition (ops/voxel_pooling/src/voxel_pooling_forward_cuda.cu:38,

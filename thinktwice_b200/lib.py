@@ -154,6 +154,13 @@ class InterpBilinearTrainDesc(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('N', 'C', 'H', 'W', 'OH', 'OW', 'align_corners')]
 
 
+class BatchNormTrainDesc(C.Structure):
+    """tt_batch_norm_train_desc (include/tt_b200.h section 18): rows, channels, ranks and options of one training-side batch norm."""
+    _fields_ = [('M', C.c_longlong), ('count', C.c_longlong)] + \
+               [(n, C.c_int) for n in ('C', 'R', 'affine', 'track_running_stats', 'training', 'residual', 'act')] + \
+               [('eps', C.c_double), ('factor', C.c_double)]
+
+
 _lib = None
 
 
@@ -172,7 +179,7 @@ def load():
               'tt_rulebook_workspace_bytes', 'tt_conv2d_workspace_bytes', 'tt_loss_workspace_bytes', 'tt_camera_loss_workspace_bytes',
               'tt_deform_conv_workspace_bytes', 'tt_sparse_conv_train_workspace_bytes', 'tt_sparse_pairs_ordered_workspace_bytes',
               'tt_lift_splat_train_workspace_bytes', 'tt_loss_backward_workspace_bytes', 'tt_camera_loss_train_workspace_bytes',
-              'tt_conv2d_train_workspace_bytes', 'tt_conv_transpose2d_train_workspace_bytes'):
+              'tt_conv2d_train_workspace_bytes', 'tt_conv_transpose2d_train_workspace_bytes', 'tt_batch_norm_train_workspace_bytes'):
         getattr(lib, n).restype = C.c_size_t
     if os.environ.get('TT_DEBUG'):                               # kernel-experiment knobs (tt_debug_set) for whole test / bench runs
         check(lib.tt_debug_set(int(os.environ['TT_DEBUG'], 0)), 'tt_debug_set')
@@ -198,6 +205,8 @@ EXPORTS = [
     'tt_conv2d_train_workspace_bytes', 'tt_conv2d_train_forward', 'tt_conv2d_train_backward',
     'tt_conv_transpose2d_train_workspace_bytes', 'tt_conv_transpose2d_train_forward', 'tt_conv_transpose2d_train_backward',
     'tt_interp_bilinear_train_forward', 'tt_interp_bilinear_train_backward',
+    'tt_batch_norm_train_workspace_bytes', 'tt_batch_norm_train_stats', 'tt_batch_norm_train_fold', 'tt_batch_norm_train_forward',
+    'tt_batch_norm_train_backward_reduce', 'tt_batch_norm_train_backward',
 ]
 
 
